@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""bench.py -- Llama-3-8B Q4_K_M decode (tg) through the drop-in boundary, on B200.
+"""bench.py -- Llama-3-8B Q4_K_M decode (tg) through the drop-in boundary, on H100 (sm_90a).
 
 Workload ("llama3-8b-q4_k_m-tg"): BASELINE.json configs[1].  A random-init Llama-3-8B GGUF with llama-quant.cpp's
 Q4_K_M type mix (synthetic valid blocks, 4.91 GB; tools/make_gguf.py) is loaded by the REFERENCE's unmodified libllama
-(host/_ref, built by host/Makefile) which dlopen()s our backend through GGML_BACKEND_PATH, exactly as llama-bench
+(oracle/_ref/host, built by oracle/host.mk) which dlopen()s our backend through GGML_BACKEND_PATH, exactly as llama-bench
 would; one step = one decoded token (llama_decode of 1 token + llama_synchronize -- llama-bench's test_gen loop,
 tools/llama-bench/llama-bench.cpp:2143-2162).  Every token streams the 4.6165 GB of mat-mul weights once
-(SURVEY.md section 8d), far more than the 126 MB L2, so no L2 flush is needed between steps.
+(SURVEY.md section 8d), far more than the 50 MB L2, so no L2 flush is needed between steps.
 
   value      tokens/s with everything resident on the device: the captured CUDA graph of one decode token is replayed
              K times between two CUDA events on the backend's stream (ggml_b200_replay_last_graph)
@@ -16,12 +16,16 @@ tools/llama-bench/llama-bench.cpp:2143-2162).  Every token streams the 4.6165 GB
   roofline   dominant kernel = decode_flow_kernel, the persistent dataflow decode kernel: ONE launch streams the whole token's
              4.6165 GB of mat-mul weights (32 layers + the output head), so the kernel IS the step; achieved = algorithmic bytes /
              the CUDA-event time of the replay; traffic = dram read+write of that launch from the committed ncu capture
-             (profiles/r02_flow_ncu.json), null until one exists for the current kernel
+             (profiles/r02_flow_ncu.json); none is committed, so it is null
   roofline_step   whole-token algorithmic bytes / device step time (the north-star's 0.70x target is this one)
-  llama_bench     the reference's UNMODIFIED llama-bench (host/_ref/llama-bench -p 2048 -n 128 -ub 2048 -fa 1 -r 3) on the same
+  llama_bench     the reference's UNMODIFIED llama-bench (oracle/_ref/host/llama-bench -p 2048 -n 128 -ub 2048 -fa 1 -r 3) on the same
              GGUF through the same plugin, run after the timed region: the metric as SURVEY 8(d) defines it
-  pp2048     prefill through the same API (llama-bench's test_prompt, -ub 2048) + the tcgen05 GEMM's achieved TFLOP/s
+  pp2048     prefill through the same API (llama-bench's test_prompt, -ub 2048) + the wgmma GEMM's achieved TFLOP/s
   cpu_baseline    the reference CPU backend (same libllama, n_gpu_layers = 0, all host threads) on a bounded sample
+
+--dump-outputs DIR writes the logits of the last timed step (what llama_decode hands its caller for that token, re-read from
+the device after the replay leg) as DIR/logits.npy, float32 [n_vocab].  The GGUF and the token ids are seeded, so two builds run
+with the same arguments can be compared output for output.
 
 N > 1: llama.cpp's tensor parallelism (-sm tensor, meta backend) is single-process: rank 0 drives all N GPUs through our
 ggml_backend_comm_* hooks (default: one-shot NVLink all-reduce between per-GPU programs of the persistent kernel), the other
@@ -41,7 +45,8 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 PLUGIN = os.path.join(ROOT, "llama.cpp_b200", "libggml-b200.so")
-HOSTLIB = os.path.join(ROOT, "tools", "libllama_host.so")
+HOST_DIR = os.path.join(ROOT, "oracle", "_ref", "host")   # the reference's host programs + our driver over its API
+HOSTLIB = os.path.join(HOST_DIR, "libllama_host.so")
 ALG_BYTES_PER_TOKEN = 4.6165e9        # SURVEY.md section 8(d)
 ALG_FLOP_PER_PP_TOKEN = 13.96e9
 Q4_K = 12
@@ -49,16 +54,16 @@ N_CTX = 4096                          # both arms
 
 
 def peaks():
-    """(HBM GB/s, bf16 TFLOP/s burst, bf16 TFLOP/s sustained, source)"""
+    """(HBM GB/s, bf16 TFLOP/s burst, bf16 TFLOP/s sustained, source): data-sheet denominators unless measured peaks are given"""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j["hbm_gbs"]), float(j["bf16_tflops"]), float(j.get("bf16_tflops_sustained", j["bf16_tflops"])), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, 1590.0, 1400.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, 989.0, 989.0, "NVIDIA H100 SXM data sheet (dense, 700 W)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, index: int):
         self.index, self.rows, self.proc = index, [], None
@@ -103,7 +108,7 @@ def ensure_gguf():
 
 def host_lib():
     if not os.path.exists(HOSTLIB):
-        raise SystemExit(f"bench.py: {HOSTLIB} missing (run __graft_entry__.build() where /root/reference exists)")
+        raise SystemExit(f"bench.py: {HOSTLIB} missing (run __graft_entry__.build() where the reference sources exist)")
     L = C.CDLL(HOSTLIB)
     L.lh_open.restype = C.c_void_p
     L.lh_open.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_char_p]
@@ -168,15 +173,15 @@ def flow_traffic():
 
 def llama_bench_leg(gguf):
     """The reference's unmodified llama-bench on the same GGUF through the same plugin (not inside the timed region)."""
-    exe = os.path.join(ROOT, "host", "_ref", "llama-bench")
+    exe = os.path.join(HOST_DIR, "llama-bench")
     if not os.path.exists(exe):
-        return {"unavailable": "host/_ref/llama-bench not built"}
+        return {"unavailable": "oracle/_ref/host/llama-bench not built"}
     env = dict(os.environ, GGML_BACKEND_PATH=PLUGIN)
     try:
         out = subprocess.run([exe, "-m", gguf, "-p", "2048", "-n", "128", "-ub", "2048", "-fa", "1", "-r", "3", "-o", "jsonl"], env=env, capture_output=True, text=True, timeout=300)
     except subprocess.TimeoutExpired:
         return {"unavailable": "timeout"}
-    res = {"cmd": "host/_ref/llama-bench -p 2048 -n 128 -ub 2048 -fa 1 -r 3 (GGML_BACKEND_PATH=libggml-b200.so)"}
+    res = {"cmd": "oracle/_ref/host/llama-bench -p 2048 -n 128 -ub 2048 -fa 1 -r 3 (GGML_BACKEND_PATH=libggml-b200.so)"}
     for ln in out.stdout.splitlines():
         try:
             j = json.loads(ln)
@@ -269,7 +274,12 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-pp", action="store_true")
     ap.add_argument("--no-llama-bench", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's logits to DIR/logits.npy (float32)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and args.gpus != 1:
+        ap.error("--dump-outputs needs --gpus 1 (the logits are re-read after the single-GPU replay leg)")
     if args.impl == "reference":
         return run_reference(args)
 
@@ -288,10 +298,11 @@ def main():
     if not os.path.exists(PLUGIN):
         raise SystemExit(f"bench.py: {PLUGIN} missing -- refusing to fall back to anything else")
     os.environ["GGML_BACKEND_PATH"] = PLUGIN
+    L = host_lib()                     # first: it loads the host's libggml-base.so, which the plugin names by soname
     plug = C.CDLL(PLUGIN, mode=C.RTLD_GLOBAL)
     plug.ggml_backend_score.restype = C.c_int
     if plug.ggml_backend_score() <= 0:
-        raise SystemExit("bench.py: the B200 backend reports no usable sm_100 device -- refusing to fall back to anything else")
+        raise SystemExit("bench.py: the backend reports no usable sm_90 device -- refusing to fall back to anything else")
     plug.ggml_b200_replay_last_graph.argtypes = [C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_ulonglong)]
     plug.ggml_b200_stats.argtypes = [C.POINTER(C.c_ulonglong)] * 3
     plug.ggml_b200_reread_last_output.restype = C.c_ulonglong
@@ -303,7 +314,6 @@ def main():
         plug.ggml_b200_stats(C.byref(a), C.byref(b), C.byref(c))
         return a.value, b.value, c.value
 
-    L = host_lib()
     W = max(3, args.warmup)
     K = args.steps
     devs = ",".join(f"B200{i}" for i in range(world)).encode() if world > 1 else None
@@ -351,12 +361,21 @@ def main():
             raise SystemExit(f"bench.py: the replayed graph does not reproduce the end-to-end step's logits: {replay_check}")
         plug.ggml_b200_replay_last_graph(K, C.byref(ms), C.byref(per))
         ms_dev = float(ms.value)
+        if args.dump_outputs:
+            last = np.empty(nv, np.float32)
+            if plug.ggml_b200_reread_last_output(last.ctypes.data, C.c_ulonglong(last.nbytes)) != last.nbytes:
+                raise SystemExit("bench.py: could not re-read the last timed step's logits")
+            os.makedirs(args.dump_outputs, exist_ok=True)
+            np.save(os.path.join(args.dump_outputs, "logits.npy"), last)
         tok_s = K / (ms_dev * 1e-3)
         launches = int(per.value) * K
     else:
         ms_dev = sec_e2e * 1e3
         tok_s = tok_s_e2e
         launches = l1 - l0
+        if args.dump_outputs:
+            sampler.stop()
+            raise SystemExit("bench.py: --dump-outputs needs the single-GPU replay leg")
     clocks = sampler.stop()
 
     # ---- prefill pp2048 through the same API
@@ -380,7 +399,7 @@ def main():
         "ms_per_step": ms_dev / K, "higher_is_better": True, "scaling": "strong", "vs_baseline": None,
         "dtype": "int8 x int4/6 -> int32, fp32 accumulate", "data": "synthetic random-init GGUF (Q4_K_M type mix), random token ids",
         "config": {"workload": "llama3-8b-q4_k_m-tg", "batch": 1, "n_ctx": 4096, "kv_tokens_during_timing": f"{W}..{W + K}",
-                   "host": "reference libllama (host/_ref) + GGML_BACKEND_PATH=libggml-b200.so", "flash_attn": True,
+                   "host": "reference libllama (oracle/_ref/host) + GGML_BACKEND_PATH=libggml-b200.so", "flash_attn": True,
                    "parallelism": f"-sm tensor x{world} (meta backend + ggml_backend_comm_* hooks)" if world > 1 else "single GPU",
                    "l2": "4.6 GB of weights streamed per step, larger than L2; no flush needed",
                    # N = 1: the captured graph of one token is what the replay leg times.  N > 1: every per-GPU segment between two all-reduces
@@ -418,7 +437,7 @@ def main():
             tf, ms_g = gemm_tflops()
             # the GEMM is timed alone over a few ms: the BURST cuBLAS figure is its denominator; the pp2048 step runs ~100 ms inside a
             # longer job: the SUSTAINED figure is its denominator.  Both fractions are given for both.
-            pp["gemm_roofline"] = {"bound": "tensor", "kernel": "gemm_q_tcgen05 Q4_K 14336x2048x4096 (+ activation pre-pass)", "achieved": tf,
+            pp["gemm_roofline"] = {"bound": "tensor", "kernel": "gemm_q_wgmma Q4_K 14336x2048x4096 (+ activation pre-pass)", "achieved": tf,
                                    "peak": tf_burst, "unit": "TFLOP/s", "frac": tf / tf_burst, "frac_of_sustained": tf / tf_peak, "ms_per_launch": ms_g,
                                    "peak_kind": "burst"}
             ach_pp = ALG_FLOP_PER_PP_TOKEN * pp["value"] / 1e12

@@ -1,5 +1,5 @@
 /*
- * b200_qmm.h -- C ABI of libb200qmm.so: the B200 (sm_100a) implementation of ggml's quantised mat-mul hot path.
+ * b200_qmm.h -- C ABI of libb200qmm.so: the H100 (sm_90a) implementation of ggml's quantised mat-mul hot path.
  *
  * This is the kernel-level boundary.  The reference-facing drop-in boundary (the ggml backend plugin that stock
  * llama.cpp binaries dlopen through GGML_BACKEND_PATH) is declared in include/ggml-b200.h and is a thin C++ layer
@@ -11,7 +11,7 @@
  *   - *_dev pointers are CUDA device pointers on the current device; `stream` is a cudaStream_t passed as void*
  *     (NULL = default stream).  All calls are asynchronous on `stream` unless stated otherwise.
  *   - return value: 0 on success, otherwise a negative B200_E_* code; b200_qmm_last_error() gives the text.
- *     There is no CPU fallback: without a usable sm_100 device every compute call fails with B200_E_NO_DEVICE.
+ *     There is no CPU fallback: without a usable sm_90 device every compute call fails with B200_E_NO_DEVICE.
  *   - matrix layout is ggml's (ggml/include/ggml.h:1425-1431): weight src0 = [K, M] quantised along K, row m at
  *     w + m*row_stride bytes; activation src1 = [K, N] f32, column n at x + n*ldx floats; dst = [M, N] f32,
  *     column n at dst + n*ldd floats.
@@ -41,12 +41,12 @@ extern "C" {
 #define B200_E_MISALIGNED   -2   /* pointer or stride violates the alignment contract above                        */
 #define B200_E_WORKSPACE    -3   /* workspace too small                                                            */
 #define B200_E_CUDA         -4   /* a CUDA call failed; see b200_qmm_last_error()                                  */
-#define B200_E_NO_DEVICE    -5   /* no sm_100 device / driver                                                      */
+#define B200_E_NO_DEVICE    -5   /* no sm_90 device / driver                                                       */
 #define B200_E_UNSUPPORTED  -6
 
 B200_API int          b200_qmm_abi_version(void);
 B200_API const char * b200_qmm_last_error(void);
-/* number of usable sm_100 devices (0 if none); never fails */
+/* number of usable sm_90 devices (0 if none); never fails */
 B200_API int          b200_qmm_device_count(void);
 
 /* ggml_row_size(type, k) (ggml/src/ggml.c): bytes of one quantised row of k weights; 0 if unsupported */
@@ -73,7 +73,7 @@ B200_API int    b200_act_layout(int weight_type, void * ws_dev, int64_t n, int64
 B200_API void   b200_set_q8_0_rounding(int mode);
 
 /* ---- replaces ggml_compute_forward_mul_mat for quantised src0 (ggml/src/ggml-cpu/ggml-cpu.c:1254-1452) ----
- * dst[M,N] = W[M,K] . X[K,N].  N <= 8 runs the decode GEMV (mmvq regime, ggml-cuda/mmvq.cu), N > 8 the tcgen05
+ * dst[M,N] = W[M,K] . X[K,N].  N <= 8 runs the decode GEMV (mmvq regime, ggml-cuda/mmvq.cu), N > 8 the wgmma
  * prefill GEMM (mmq regime, ggml-cuda/mmq.cu).  ws_dev >= b200_mul_mat_workspace_bytes(). */
 B200_API size_t b200_mul_mat_workspace_bytes(int type, int64_t M, int64_t N, int64_t K);
 B200_API int    b200_mul_mat(int type, const void * w_dev, int64_t row_stride, int64_t M, int64_t K,
@@ -112,8 +112,6 @@ B200_API size_t b200_flow_slot_bytes(void);
 B200_API void   b200_set_mul_mat_path(int path);
 /* decode kernel generation: 2 = block-per-lane bulk-copy kernel where it applies (default), 1 = first generation */
 B200_API void   b200_set_gemv_variant(int variant);
-/* prefill kernel generation: 2 = warp-specialised, pipelined tcgen05 kernel (default), 1 = first generation (serial phases) */
-B200_API void   b200_set_gemm_variant(int variant);
 
 /* ---- replaces ggml_compute_forward_mul_mat_id (ggml/src/ggml-cpu/ggml-cpu.c:1534-1707) ----
  * as = [K, M, n_expert] (expert e at w_dev + e*expert_stride), b = [K, nb1, T] f32 contiguous (nb1 = n_used or 1),

@@ -9,7 +9,7 @@
  *   export GGML_BACKEND_PATH=/path/to/libggml-b200.so      # ggml_backend_load_all() dlopens it (reg.cpp:566-593)
  *   llama-bench -m model.gguf -ngl 99 -fa 1 [-sm tensor]   # unmodified reference binaries
  *
- * Registry "B200"; devices "B2000".."B200<n-1>" (one per sm_100 GPU, type GPU, caps async + events); buffer type per
+ * Registry "B200"; devices "B2000".."B200<n-1>" (one per sm_90 GPU, type GPU, caps async + events); buffer type per
  * device (cudaMalloc, 128-byte tensor alignment, native GGUF block layout); backend = one CUDA stream.
  * get_proc_address() answers: ggml_backend_comm_init / ggml_backend_comm_free / ggml_backend_comm_allreduce_tensor
  * (ggml/include/ggml-backend.h:208-210, used by the meta backend for -sm tensor) and ggml_backend_get_features.
@@ -28,7 +28,7 @@ struct ggml_backend_reg;
 
 /* required dl entry point (ggml_backend_init_t): returns the registry object, api_version = GGML_BACKEND_API_VERSION (2) */
 struct ggml_backend_reg * ggml_backend_init(void);
-/* optional dl entry point (ggml_backend_score_t): 0 when no sm_100 device is usable (the loader then skips the plugin) */
+/* optional dl entry point (ggml_backend_score_t): 0 when no sm_90 device is usable (the loader then skips the plugin) */
 int ggml_backend_score(void);
 
 /* ---- measurement hooks used by bench.py; not part of the ggml interface ---- */

@@ -1,13 +1,13 @@
 // ggml_b200.cpp -- the drop-in boundary: an out-of-tree ggml backend ("B200") implementing the reference's five
 // plugin vtables (ggml/src/ggml-backend-impl.h:17-230) and the dl entry points ggml_backend_init / ggml_backend_score
 // (:232-271) so that unmodified llama.cpp hosts (llama-bench, llama-cli, test-backend-ops, libllama) load it through
-// GGML_BACKEND_PATH (ggml-backend-reg.cpp:566-593) and run GGUF models on sm_100a.
+// GGML_BACKEND_PATH (ggml-backend-reg.cpp:566-593) and run GGUF models on sm_90a (H100).
 //
 // Host-side C++ only: tensors are mapped onto plain views / pointers and handed to the hand-written CUDA in ../csrc
 // (the same objects that make up libb200qmm.so).  Built from scratch against the interface; ggml-cuda is not ported.
 //
 //   reg      B200        get_proc_address: ggml_backend_comm_{init,free,allreduce_tensor} (meta backend, -sm tensor)
-//   device   B2000..N    one per sm_100 GPU; GPU type; async + events
+//   device   B2000..N    one per sm_90 GPU; GPU type; async + events
 //   buft     B200<i>     cudaMalloc'd buffers, 128-byte tensor alignment, 256 bytes of tail slack for 16-byte loads
 //   backend  one CUDA stream; graph_compute enqueues every node and returns without blocking; graphs whose
 //            cgraph->uid repeats are captured once into a CUDA graph and replayed
@@ -493,7 +493,7 @@ cudaError_t run_mul_mat_id(backend_ctx * b, const ggml_tensor * node) {
     const ggml_tensor * w = node->src[0], * x = node->src[1], * ids = node->src[2];
     const int type = (int)w->type;
     const int64_t K = w->ne[0], M = w->ne[1], n_expert = w->ne[2], nb1 = x->ne[1], T = x->ne[2], n_used = ids->ne[0];
-    // many (token, slot) rows: group them by expert and run the tcgen05 GEMM once per expert tile (the per-row GEMV below would stream
+    // many (token, slot) rows: group them by expert and run the wgmma GEMM once per expert tile (the per-row GEMV below would stream
     // an expert's weights once per row)
     static const bool no_grouped = getenv("GGML_B200_NO_GROUPED_GEMM") != nullptr;
     if (!no_grouped && T * n_used >= 32 && qmm::gemm_grouped_workspace_bytes(type, M, T * n_used, n_expert, K) != 0) {
@@ -551,7 +551,7 @@ inline bool decode_mm_ok(const ggml_tensor * n) {
 void find_next_weights(const ggml_cgraph * g, int from, qmm::FusedGemvArgs & a) {
     static const bool enabled = getenv("GGML_B200_L2_PREFETCH") != nullptr;   // opt-in: measured slightly negative (it queues ahead of demand loads)
     if (!enabled) return;
-    int64_t budget = 80ll << 20;                                   // leave room in the 126 MB L2 for the current stream
+    int64_t budget = 32ll << 20;                                   // leave room in the 50 MB L2 for the current stream
     for (int j = from; j < g->n_nodes; j++) {
         const ggml_tensor * n = g->nodes[j];
         if (is_noop(n) || !decode_mm_ok(n)) continue;
@@ -1649,7 +1649,7 @@ size_t reg_dev_count(ggml_backend_reg_t) { return g_devices.size(); }
 ggml_backend_dev_t reg_get_device(ggml_backend_reg_t, size_t i) { return i < g_dev_objs.size() ? &g_dev_objs[i] : nullptr; }
 
 ggml_backend_feature * reg_features(ggml_backend_reg_t) {
-    static ggml_backend_feature f[] = {{"ARCH", "sm_100a"}, {"TCGEN05", "1"}, {"CPU_FALLBACK", "0"}, {nullptr, nullptr}};
+    static ggml_backend_feature f[] = {{"ARCH", "sm_90a"}, {"WGMMA", "1"}, {"CPU_FALLBACK", "0"}, {nullptr, nullptr}};
     return f;
 }
 
@@ -1669,7 +1669,7 @@ void init_registry() {
     for (int i = 0; i < n && (int)g_devices.size() < MAX_DEVICES; i++) {
         cudaDeviceProp p;
         if (cudaGetDeviceProperties(&p, i) != cudaSuccess) { cudaGetLastError(); continue; }
-        if (p.major != 10) continue;                       // sm_100a code only: no other architecture, no fallback
+        if (p.major != 9) continue;                        // sm_90a code only: no other architecture, no fallback
         auto * d = new device_ctx();
         d->index = (int)g_devices.size();
         d->cuda_dev = i;

@@ -1,5 +1,5 @@
-"""In-tree build of the product's shared objects (nvcc, sm_100a).  No JIT cache: the .so files sit next to the
-sources so that they travel to the GPU box with the repo snapshot."""
+"""In-tree build of the product's shared objects (nvcc, sm_90a).  No JIT cache: the .so files sit next to the
+sources, so the package is importable from the repository tree."""
 from __future__ import annotations
 
 import os
@@ -9,6 +9,7 @@ PKG = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(PKG)
 LIB_QMM = os.path.join(PKG, "libb200qmm.so")
 LIB_PLUGIN = os.path.join(PKG, "libggml-b200.so")
+BACKEND = os.path.join(PKG, "backend")
 
 
 def build_kernels(jobs: int = 8) -> str:
@@ -16,20 +17,12 @@ def build_kernels(jobs: int = 8) -> str:
     return LIB_QMM
 
 
-def build_plugin(jobs: int = 8) -> str | None:
-    """The plugin compiles against the reference's headers (ggml-backend-impl.h); it can only be (re)built where
-    /root/reference exists.  On the GPU box the prebuilt .so is used."""
-    mk = os.path.join(PKG, "backend", "Makefile")
-    if not os.path.exists(mk):
-        return None
-    if not os.path.isdir("/root/reference"):
-        return LIB_PLUGIN if os.path.exists(LIB_PLUGIN) else None
-    # the plugin names the reference HOST's libggml-base (host/_ref) as DT_NEEDED, so that has to exist first
-    subprocess.check_call(["make", "-s", f"-j{jobs}", "-C", os.path.join(ROOT, "host"), "libs"])
-    subprocess.check_call(["make", "-s", f"-j{jobs}", "-C", os.path.join(PKG, "backend")])
+def build_plugin_objects(objdir: str, ref: str, jobs: int = 8) -> None:
+    """The plugin's C++ objects compile against the reference's internal ggml headers: only where those sources exist."""
+    subprocess.check_call(["make", "-s", f"-j{jobs}", "-C", BACKEND, "objs", f"OBJDIR={objdir}", f"REF={ref}"])
+
+
+def link_plugin(objdir: str, hostlib: str, jobs: int = 8) -> str:
+    """Compiles the kernels and links them with the plugin's C++ objects (objdir) against the host's libggml-base (hostlib)."""
+    subprocess.check_call(["make", "-s", f"-j{jobs}", "-C", BACKEND, "link", f"OBJDIR={objdir}", f"HOSTLIB={hostlib}"])
     return LIB_PLUGIN
-
-
-def build_all() -> None:
-    build_kernels()
-    build_plugin()

@@ -1,6 +1,6 @@
 // allreduce.cu -- one-shot NVLink all-reduce for the tensor-parallel decode path (messages of tens of KB).
 //
-// Every GPU owns a symmetric buffer, peer-mapped by all others (cudaDeviceEnablePeerAccess; on an HGX B200 every pair
+// Every GPU owns a symmetric buffer, peer-mapped by all others (cudaDeviceEnablePeerAccess; on an HGX H100 every pair
 // is one NVSwitch hop).  For call number `seq` (kept in device memory, so the launch is CUDA-graph capturable):
 //   1. rank r copies its vector into slot r of EVERY rank's buffer set (seq & 1)   -- peer stores over NVLink
 //   2. __threadfence_system(), then rank r writes seq into flag[r] of every rank    -- release

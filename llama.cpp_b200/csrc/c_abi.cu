@@ -54,7 +54,7 @@ int b200_qmm_device_count(void) {
     int ok = 0;
     for (int i = 0; i < n; i++) {
         int major = 0;
-        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 10) ok++;
+        if (cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, i) == cudaSuccess && major == 9) ok++;
     }
     return ok;
 }
@@ -87,7 +87,6 @@ int b200_act_layout(int wt, void * ws, int64_t n, int64_t k, void ** qs, void **
 void b200_set_q8_0_rounding(int mode) { set_q8_0_mode(mode); }
 void b200_set_mul_mat_path(int path) { g_path = path; }
 void b200_set_gemv_variant(int v) { set_gemv_variant(v); }
-void b200_set_gemm_variant(int v) { set_gemm_variant(v); }
 
 size_t b200_mul_mat_workspace_bytes(int type, int64_t M, int64_t N, int64_t K) {
     if (!type_ok(type)) return 0;
@@ -214,7 +213,7 @@ int b200_flow_selftest_postponed_rope(void) {
     static uint64_t pool[1 << 16];
     const uintptr_t fake = 0x100000;
     FlowBuilder fb;
-    fb.reset(pool, sizeof(pool) / sizeof(pool[0]), 148);
+    fb.reset(pool, sizeof(pool) / sizeof(pool[0]), 132);
     float * A = (float *)(fake * 1), * C = (float *)(fake * 2), * X = (float *)(fake * 3), * OUT = (float *)(fake * 4);
     FlowBuilder::MatvecDesc q;
     q.nmat = 1; q.K = 4096; q.mode = 0; q.w[0] = (const uint8_t *)(fake * 8); q.row_stride[0] = 16 * 144; q.M[0] = 4096; q.type[0] = T_Q4_K; q.dst[0] = A;

@@ -814,6 +814,13 @@ __device__ __forceinline__ void consume_matrix(const MatCtx & mc, int nch, unsig
         const int ch = mc.S == 1 ? t : t >> 1, sgm = mc.S == 1 ? 0 : t & 1;
         const unsigned g = gbase + qbase + (unsigned)t, slot = g % FL_NSLOTS, use = g / FL_NSLOTS;
         const long long tw0 = timed ? clock64() : 0;
+        // The warps take pieces round-robin, so the consumer of the slot's previous use is another warp, and this warp can get here while
+        // that use's copy is still landing.  A parity wait on `full` alone would then see the phase before it (same parity) and pass.  Wait
+        // first for the previous use to be released.  That wait cannot alias: every mat-vec phase starts with a barrier of all consumer
+        // warps, and inside a phase a warp takes every FL_NW-th (S == 2: every 2 FL_NPAIR-th) piece, so this warp's previous piece is fewer
+        // than FL_NSLOTS pieces back -- then it, and before it the slot's previous use, were issued, which the producer did only after the
+        // use before was released -- or the previous use lies before this phase and was consumed at that barrier.
+        if (use > 0) fl_mbar_wait(empty + slot, (use - 1) & 1u);
         fl_mbar_wait(full + slot, use & 1u);
         const long long tw1 = timed ? clock64() : 0;
         const int r0 = mc.rb + ch * mc.R;
@@ -1443,7 +1450,7 @@ int sm_count_of(int dev) {
     static int cnt[64] = {};
     dev &= 63;
     if (!cnt[dev]) {
-        int n = 148;
+        int n = 132;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
         cnt[dev] = n;
     }
@@ -1506,7 +1513,7 @@ void FlowBuilder::reset(uint64_t * ll_pool, size_t ll_elems, int grid) {
     produced_.clear();
     h_ptr_ = nullptr; h_ptr_copy_ = nullptr;
     pool_ = ll_pool; pool_elems_ = ll_elems; head_ = 0; seg_start_ = 0; n_coll_ = 0;
-    grid_ = grid > 0 ? grid : 148;
+    grid_ = grid > 0 ? grid : 132;
 }
 
 void FlowBuilder::cut() {

@@ -165,7 +165,7 @@ private:
     uint64_t * pool_ = nullptr;
     size_t pool_elems_ = 0, head_ = 0, seg_start_ = 0;
     int n_coll_ = 0;
-    int grid_ = 148;
+    int grid_ = 132;
     uint64_t * carve(size_t n);
 };
 

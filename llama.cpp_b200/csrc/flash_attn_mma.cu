@@ -4,7 +4,7 @@
 //
 // This is a supporting op of the mat-mul path (SURVEY.md section 8f rank 1), not the headline kernel: at pp2048 its
 // FLOPs are 4 % of the weight GEMMs'.  It uses warp-level mma.sync.m16n8k16 (f16 x f16 -> f32), which is enough to take
-// attention from 60 % of the prefill step (scalar kernel in ops.cu) to a few per cent; the tcgen05 budget goes to the
+// attention from 60 % of the prefill step (scalar kernel in ops.cu) to a few per cent; the wgmma budget goes to the
 // quantised GEMM (gemm_tcgen05.cu).
 //
 // Shape: one CTA = 4 warps = 64 query rows of one head; KV tiles of 64 keys double-buffered with cp.async (L2 only: .cg).

@@ -1,7 +1,7 @@
 // gemm_layout.cuh -- operand images of the prefill GEMM (gemm_tcgen05.cu), shared by the activation pre-pass, the
 // weight de-quantiser and the host-side layout test (tests/host_gemm_layout.cpp).
 //
-// tcgen05.mma kind::f16 consumes K-major operands from shared memory in the canonical SWIZZLE_128B layout:
+// wgmma.mma_async (fp16) consumes K-major operands from shared memory in the canonical SWIZZLE_128B layout:
 // an "atom" is ROWS x 64 fp16 (128 bytes per row); rows are stored in groups of 8 (1024 bytes); inside a group the
 // 16-byte chunk index is XORed with the row index (Swizzle<3,4,3>).  One 256-weight K block = 4 atoms.
 //

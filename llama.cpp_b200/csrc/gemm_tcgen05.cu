@@ -1,4 +1,4 @@
-// gemm_tcgen05.cu -- prefill GEMM for K-quant weights on the 5th-generation tensor cores:
+// gemm_tcgen05.cu -- prefill GEMM for K-quant weights on the sm_90a warpgroup tensor cores (wgmma; the file name is historical):
 //     dst[M, N] = W[M, K] . X[K, N],   N > 8      (the mmq regime of ggml_compute_forward_mul_mat, ggml-cpu.c:1254-1452;
 //                                                  closest analogue in the reference: mul_mat_q, ggml-cuda/mmq.cuh:946-1231)
 //
@@ -8,19 +8,18 @@
 //   integers, exactly representable in fp16:
 //       A  = sc_j * q_w      (<= 63*15 for Q4_K, 63*31 for Q5_K)      B  = q_a (the CPU-identical Q8_K integers)
 //       A' = m_j             (6 bit)                                    B' = bsum_j split into (even part, low bit)
-//   tcgen05.mma kind::f16 accumulates them in fp32 in TMEM (exact below 2^24).  After every K block the accumulator
-//   tile is drained from TMEM (tcgen05.ld) and combined in registers with the block's fp16/fp32 scales:
+//   wgmma.mma_async accumulates them in fp32 registers (exact below 2^24).  After every K block the block's integer sums are
+//   combined in registers with the block's fp16/fp32 scales:
 //       acc += (d_w d_a) * main - (dmin_w d_a) * mins
-//   i.e. the same per-block fp32 combine the CPU does.
+//   i.e. the same per-block fp32 combine the CPU does (the mins term is added first).
 //
-// This file is generation 1 of the kernel: one CTA per 128 x 128 output tile, cta_group::1, operands staged in shared
-// memory (weights de-quantised on the fly by all 8 warps into the canonical 128B-swizzled K-major layout, activations
-// pre-packed into that layout by quantize_act_gemm_kernel and brought in with one cp.async.bulk per K block), one
-// elected thread issues the 17 MMAs of a block, tcgen05.commit signals an mbarrier, all warps drain TMEM.  The phases of
-// a K block still run back to back (no overlap yet): see DESIGN.md for the measured tensor-pipe fraction and the plan
-// (TMEM-resident A, double-buffered accumulators, warp specialisation, cta_group::2).
+// Structure: one CTA of two warpgroups per 128 x 128 output tile; warpgroup g owns weight rows 64 g .. 64 g + 63 of the tile.
+// Per K block, thread 0 starts one bulk copy of the activation image (written in the canonical 128B-swizzled K-major layout by
+// quantize_act_gemm_kernel) while every warpgroup de-quantises ITS rows of the weight block into the same layout; a warpgroup then
+// waits only for its own rows and the activation copy, issues its m64n128k16 MMAs and rescales.  The two warpgroups meet only at
+// the activation buffer (an mbarrier that counts both out before the next copy), so one de-quantises while the other multiplies.
 //
-// Algorithmic FLOPs per launch: 2 M N K.  Roofline: bf16/fp16 tensor pipe.
+// Algorithmic FLOPs per launch: 2 M N K.  Roofline: fp16 tensor pipe.
 #include <cuda_fp16.h>
 #include <stdlib.h>
 
@@ -33,20 +32,17 @@ namespace qmm {
 
 constexpr int GEMM_NT      = 128;                 // token columns per CTA tile
 constexpr int GEMM_MT      = 128;                 // weight rows per CTA tile
-constexpr int GEMM_THREADS = 256;
+constexpr int GEMM_THREADS = 256;                 // two warpgroups, 64 weight rows each
 
 static inline int64_t rup(int64_t v, int64_t a) { return (v + a - 1) / a * a; }
 
 // workspace: [B images: ntiles x nkb x bimg_block_bytes] [d_a: nkb x Npad floats]
-constexpr int GEMM_NT3 = 192;                // token columns per CTA tile of the generation-3 kernel
 size_t gemm_workspace_bytes(int type, int64_t M, int64_t N, int64_t K) {
     if (type == T_Q4_0 || type == T_Q8_0) return gemm_legacy_workspace_bytes(type, M, N, K);
     if (!(type == T_Q4_K || type == T_Q5_K || type == T_Q6_K) || K % 256 || N <= 0) return 0;
     const int64_t nkb = K / 256;
-    const int64_t npad = rup(N, GEMM_NT), npad3 = rup(N, GEMM_NT3);
-    const size_t a = (size_t)(npad / GEMM_NT * nkb * gl::bimg_block_bytes(GEMM_NT) + nkb * npad * 4 + 1024);
-    const size_t b = (size_t)(npad3 / GEMM_NT3 * nkb * gl::bimg_block_bytes(GEMM_NT3) + nkb * npad3 * 4 + 1024);
-    return a > b ? a : b;                     // the images of either tile width fit
+    const int64_t npad = rup(N, GEMM_NT);
+    return (size_t)(npad / GEMM_NT * nkb * gl::bimg_block_bytes(GEMM_NT) + nkb * npad * 4 + 1024);
 }
 
 // ------------------------------------------------------------------------------------------------ activation pre-pass
@@ -193,7 +189,7 @@ __device__ __forceinline__ void dequant_block_to_smem(const uint8_t * __restrict
 
 // Q6_K: x = d * sc * (q - 32), sc int8, q 6 bit.  |sc (q-32)| reaches 4096 > 2048, so odd products would not be exact in
 // fp16.  Split sc = sc_even + sc_lsb (sc_lsb = sc & 1): A1 = sc_even (q-32) is even and <= 4096 (exact), A2 = sc_lsb (q-32)
-// is tiny; both tiles are multiplied with the same B and accumulated into the same TMEM tile (32 MMAs per block, no mins).
+// is tiny; both tiles are multiplied with the same B and accumulated into the same registers (32 MMAs per block, no mins).
 // Thread (row r, half h) expands weights 128h .. 128h+127 into atoms 2h (quarters 0,1) and 2h+1 (quarters 2,3).
 __device__ __forceinline__ uint32_t ldg4_a2(const uint8_t * p) {       // 4 bytes from a 2-byte aligned global address
     const uint32_t * w = reinterpret_cast<const uint32_t *>(reinterpret_cast<uintptr_t>(p) & ~uintptr_t(3));
@@ -259,830 +255,164 @@ struct GemmKArgs {
     // is written to dst column col_dst[n] (< 0: padding).  nullptr: a plain GEMM.
     const int * tile_expert; const int * col_dst; int64_t expert_stride;
 };
-__device__ __forceinline__ int gemm_dst_col(const GemmKArgs & p, int n) { return p.col_dst ? p.col_dst[n] : (n < p.N ? n : -1); }
 template <bool GROUPED> __device__ __forceinline__ int gemm_dst_col_t(const GemmKArgs & p, int n) { if constexpr (GROUPED) return p.col_dst[n]; else return n < p.N ? n : -1; }
 
-template <int T>
-__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_q_tcgen05_kernel(const GemmKArgs p) {
+template <int T> struct KqCfg {
+    static constexpr bool IS_Q6 = (T == T_Q6_K);
+    static constexpr int ATOM_A = GEMM_MT * 128, ATOM_B = GEMM_NT * 128;
+    static constexpr int A_BYTES = (IS_Q6 ? 8 : 5) * ATOM_A;      // 4 atoms + (Q6_K: 4 atoms of the odd-scale part; else 1 of mins)
+    static constexpr int B_BYTES = 5 * ATOM_B;                     // exactly one B image block (gemm_layout.cuh)
+    static constexpr size_t SMEM = 1024 + (size_t)A_BYTES + B_BYTES + 64;
+};
+
+// acc += scale(row) * d_a(col) * v over the thread's fragment (see wgmma_m64n128k16_f16 for which element each register holds)
+__device__ __forceinline__ void kq_combine(float (&acc)[64], const float (&v)[64], float s_lo, float s_hi, const float * __restrict__ dap, int c4) {
+#pragma unroll
+    for (int i = 0; i < 16; i++) {
+        const float2 da = __ldg(reinterpret_cast<const float2 *>(dap + 8 * i + 2 * c4));
+        acc[4 * i + 0] += (s_lo * da.x) * v[4 * i + 0];
+        acc[4 * i + 1] += (s_lo * da.y) * v[4 * i + 1];
+        acc[4 * i + 2] += (s_hi * da.x) * v[4 * i + 2];
+        acc[4 * i + 3] += (s_hi * da.y) * v[4 * i + 3];
+    }
+}
+
+template <int T, bool GROUPED>
+__global__ void __launch_bounds__(GEMM_THREADS, 1) gemm_q_wgmma_kernel(const GemmKArgs p) {
+    // The grouped (MUL_MAT_ID) form is its own instantiation, so that the plain GEMM carries no expert lookup.
+    const uint8_t * wbase = p.w;
+    if constexpr (GROUPED) {                               // this column tile's expert (uniform per CTA)
+        const int e = p.tile_expert[blockIdx.y];
+        if (e < 0) return;
+        wbase += (int64_t)e * p.expert_stride;
+    }
+    using C = KqCfg<T>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     uint8_t * smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    constexpr int ATOM_A = GEMM_MT * 128, ATOM_B = GEMM_NT * 128;
-    constexpr bool IS_Q6 = (T == T_Q6_K);
     uint8_t * sA = smem;                                   // 4 atoms
-    uint8_t * sAmin = sA + 4 * ATOM_A;                     // Q4_K/Q5_K: 1 atom of mins; Q6_K: 4 atoms of the odd-scale part
-    uint8_t * sB = sAmin + (IS_Q6 ? 4 : 1) * ATOM_A;       // 4 + 1 atoms, exactly one B image block
-    float * s_da = reinterpret_cast<float *>(sB + 5 * ATOM_B);
-    uint64_t * bar_b = reinterpret_cast<uint64_t *>(s_da + GEMM_NT);
-    uint64_t * bar_mma = bar_b + 1;
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(bar_mma + 1);
+    uint8_t * sAx = sA + 4 * C::ATOM_A;                    // Q4_K/Q5_K: 1 atom of mins; Q6_K: 4 atoms of the odd-scale part
+    uint8_t * sB = sA + C::A_BYTES;
+    uint64_t * bar_full = reinterpret_cast<uint64_t *>(sB + C::B_BYTES);    // bulk copy of the B block landed
+    uint64_t * bar_empty = bar_full + 1;                   // both warpgroups' MMAs have read it (256 arrivals)
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x, wg = tid >> 7, t = tid & 127;
     const int m0 = blockIdx.x * GEMM_MT, tile = blockIdx.y;
     const int nkb = p.K >> 8;
-    constexpr uint32_t TM_COLS = 2 * GEMM_NT;              // main + mins accumulators
-
-    if (tid == 0) { g_mbar_init(bar_b, 1); g_mbar_init(bar_mma, 1); asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory"); }
-    if (warp == 0) tmem_alloc(tmem_slot, TM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    const int r = tid & 127, h = tid >> 7;
-    const bool row_ok = m0 + r < p.M;
-    const uint8_t * wrow = p.w + (int64_t)(m0 + r) * p.row_stride;
     constexpr int BB = Fmt<T>::BB;
 
-    // epilogue ownership: TMEM lane = 32*(warp&3) + lane = output row; column half = warp >> 2
-    const int erow = 32 * (warp & 3) + lane, ecol0 = (warp >> 2) * (GEMM_NT / 2);
-    const bool erow_ok = m0 + erow < p.M;
-    const uint8_t * ewrow = p.w + (int64_t)(m0 + erow) * p.row_stride;
-    float acc[GEMM_NT / 2];
-#pragma unroll
-    for (int i = 0; i < GEMM_NT / 2; i++) acc[i] = 0.0f;
+    if (tid == 0) { g_mbar_init(bar_full, 1); g_mbar_init(bar_empty, GEMM_THREADS); asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory"); }
+    __syncthreads();
 
-    const uint32_t idesc_main = make_idesc_f16(GEMM_MT, GEMM_NT);
+    // de-quantiser ownership: thread (row r, half h) expands weights 128 h .. 128 h + 127 of row r (only rows of its own warpgroup)
+    const int r = 64 * wg + (t & 63), h = t >> 6;
+    const bool row_ok = m0 + r < p.M;
+    const uint8_t * wrow = wbase + (int64_t)(m0 + r) * p.row_stride;
+    // accumulator ownership: rows er, er + 8 of the tile, columns 8 i + 2 c4 (+ 1)
+    const int c4 = t & 3, er = 64 * wg + 16 * (t >> 5) + ((t & 31) >> 2);
+    const bool ok_lo = m0 + er < p.M, ok_hi = m0 + er + 8 < p.M;
+    const uint8_t * ew_lo = wbase + (int64_t)(m0 + er) * p.row_stride, * ew_hi = ew_lo + 8 * p.row_stride;
+    const uint32_t a_off = (uint32_t)wg * 64 * 128;        // this warpgroup's 64 rows inside an A atom (8 row groups of 1024 B)
+
+    float acc[64], v[64];
+#pragma unroll
+    for (int i = 0; i < 64; i++) { acc[i] = 0.0f; v[i] = 0.0f; }
     const int64_t bblk = gl::bimg_block_bytes(GEMM_NT);
 
     for (int kb = 0; kb < nkb; kb++) {
         const uint32_t par = (uint32_t)(kb & 1);
-        // (1) B image of this block: one bulk copy; d_a of the tile's tokens
+        // (1) B image of this block: one bulk copy, once both warpgroups are done with the previous one
         if (tid == 0) {
-            g_mbar_expect_tx(bar_b, (uint32_t)bblk);
-            g_bulk_g2s(sB, p.bimg + ((int64_t)tile * nkb + kb) * bblk, (uint32_t)bblk, bar_b);
+            g_mbar_wait(bar_empty, par ^ 1u);
+            g_mbar_expect_tx(bar_full, (uint32_t)bblk);
+            g_bulk_g2s(sB, p.bimg + ((int64_t)tile * nkb + kb) * bblk, (uint32_t)bblk, bar_full);
         }
-        if (tid < GEMM_NT) s_da[tid] = p.da[(int64_t)kb * p.npad + tile * GEMM_NT + tid];
-        // (2) weights -> fp16 integers in the swizzled K-major layout
-        if constexpr (IS_Q6) dequant_q6_block_to_smem(wrow + (int64_t)kb * BB, row_ok, r, h, sA, sAmin);
-        else dequant_block_to_smem<T>(wrow + (int64_t)kb * BB, row_ok, r, h, sA, sAmin);
+        // (2) this warpgroup's weight rows -> fp16 integers in the swizzled K-major layout
+        if constexpr (C::IS_Q6) dequant_q6_block_to_smem(wrow + (int64_t)kb * BB, row_ok, r, h, sA, sAx);
+        else dequant_block_to_smem<T>(wrow + (int64_t)kb * BB, row_ok, r, h, sA, sAx);
         fence_proxy_async();                                // generic-proxy smem writes -> visible to the tensor core (async proxy)
-        __syncthreads();
-        // (3) one thread issues the block's MMAs
-        if (warp == 0) {
-            g_mbar_wait(bar_b, par);
-            tc_fence_after();
-            if (lane == 0) {
-#pragma unroll
-                for (int a = 0; a < 4; a++) {
-#pragma unroll
-                    for (int ks = 0; ks < 4; ks++) {
-                        const uint64_t da_ = make_desc_sw128(s32(sA + a * ATOM_A) + ks * 32);
-                        const uint64_t db_ = make_desc_sw128(s32(sB + a * ATOM_B) + ks * 32);
-                        umma_f16(tmem_base, da_, db_, idesc_main, (a | ks) != 0 ? 1u : 0u);
-                    }
-                }
-                if constexpr (IS_Q6) {
-#pragma unroll
-                    for (int a = 0; a < 4; a++) {
-#pragma unroll
-                        for (int ks = 0; ks < 4; ks++)
-                            umma_f16(tmem_base, make_desc_sw128(s32(sAmin + a * ATOM_A) + ks * 32), make_desc_sw128(s32(sB + a * ATOM_B) + ks * 32), idesc_main, 1u);
-                    }
-                } else {
-                    umma_f16(tmem_base + GEMM_NT, make_desc_sw128(s32(sAmin)), make_desc_sw128(s32(sB + 4 * ATOM_B)), idesc_main, 0u);
-                }
-                umma_commit(bar_mma);
+        wg_bar_sync(wg);
+        float dw_lo = 0.0f, dw_hi = 0.0f, dm_lo = 0.0f, dm_hi = 0.0f;
+        if constexpr (C::IS_Q6) {
+            if (ok_lo) dw_lo = __half2float(__ushort_as_half(__ldg(reinterpret_cast<const unsigned short *>(ew_lo + (int64_t)kb * BB + 208))));
+            if (ok_hi) dw_hi = __half2float(__ushort_as_half(__ldg(reinterpret_cast<const unsigned short *>(ew_hi + (int64_t)kb * BB + 208))));
+        } else {
+            if (ok_lo) {
+                const uint32_t dd = __ldg(reinterpret_cast<const uint32_t *>(ew_lo + (int64_t)kb * BB));
+                dw_lo = __half2float(__ushort_as_half((unsigned short)(dd & 0xFFFFu)));
+                dm_lo = __half2float(__ushort_as_half((unsigned short)(dd >> 16)));
             }
-            __syncwarp();
-        }
-        // (4) everybody: wait for the accumulators, drain and rescale
-        g_mbar_wait(bar_mma, par);
-        tc_fence_after();
-        float dw = 0.0f, dm = 0.0f;
-        if (erow_ok) {
-            if constexpr (IS_Q6) {
-                dw = __half2float(__ushort_as_half(__ldg(reinterpret_cast<const unsigned short *>(ewrow + (int64_t)kb * BB + 208))));
-            } else {
-                const uint32_t dd = __ldg(reinterpret_cast<const uint32_t *>(ewrow + (int64_t)kb * BB));
-                dw = __half2float(__ushort_as_half((unsigned short)(dd & 0xFFFFu)));
-                dm = __half2float(__ushort_as_half((unsigned short)(dd >> 16)));
+            if (ok_hi) {
+                const uint32_t dd = __ldg(reinterpret_cast<const uint32_t *>(ew_hi + (int64_t)kb * BB));
+                dw_hi = __half2float(__ushort_as_half((unsigned short)(dd & 0xFFFFu)));
+                dm_hi = __half2float(__ushort_as_half((unsigned short)(dd >> 16)));
             }
         }
-        const uint32_t tlane = tmem_base + ((uint32_t)(32 * (warp & 3)) << 16);
+        const float * dap = p.da + (int64_t)kb * p.npad + tile * GEMM_NT;
+        g_mbar_wait(bar_full, par);
+        // (3) mins term: one K = 16 MMA; acc += d_a * (-dmin_w * mins)
+        if constexpr (!C::IS_Q6) {
+            acc_fence(v);
+            wgmma_fence();
+            wgmma_m64n128k16_f16(v, make_desc_sw128(s32(sAx) + a_off), make_desc_sw128(s32(sB + 4 * C::ATOM_B)), 0u);
+            wgmma_commit();
+            wgmma_wait<0>();
+            acc_fence(v);
+            kq_combine(acc, v, -dm_lo, -dm_hi, dap, c4);
+        }
+        // (4) main term: 16 MMAs (Q6_K: 32, both scale parts into the same accumulator); acc += d_a * (d_w * main)
+        acc_fence(v);
+        wgmma_fence();
 #pragma unroll
-        for (int c = 0; c < GEMM_NT / 2; c += 32) {
-            float vmain[32];
-            tmem_ld32(tlane + (uint32_t)(ecol0 + c), vmain);
-            if constexpr (IS_Q6) {
+        for (int a = 0; a < 4; a++) {
 #pragma unroll
-                for (int i = 0; i < 32; i++) acc[c + i] += (dw * s_da[ecol0 + c + i]) * vmain[i];
-            } else {
-                float vmin[32];
-                tmem_ld32(tlane + (uint32_t)(GEMM_NT + ecol0 + c), vmin);
-#pragma unroll
-                for (int i = 0; i < 32; i++) {
-                    const float da = s_da[ecol0 + c + i];
-                    acc[c + i] += (dw * da) * vmain[i] - (dm * da) * vmin[i];
-                }
+            for (int ks = 0; ks < 4; ks++) {
+                const uint64_t db_ = make_desc_sw128(s32(sB + a * C::ATOM_B) + ks * 32);
+                wgmma_m64n128k16_f16(v, make_desc_sw128(s32(sA + a * C::ATOM_A) + a_off + ks * 32), db_, (a | ks) != 0 ? 1u : 0u);
+                if constexpr (C::IS_Q6) wgmma_m64n128k16_f16(v, make_desc_sw128(s32(sAx + a * C::ATOM_A) + a_off + ks * 32), db_, 1u);
             }
         }
-        tc_fence_before();
-        __syncthreads();                                    // smem + TMEM free for the next block
+        wgmma_commit();
+        wgmma_wait<0>();
+        acc_fence(v);
+        g_mbar_arrive(bar_empty);                           // this thread's reads of B (and of its warpgroup's A rows) are done
+        kq_combine(acc, v, dw_lo, dw_hi, dap, c4);
     }
 
-    // (5) write out: dst[n*ldd + m]; for a fixed n the 32 lanes of a warp write 32 consecutive floats
-    if (erow_ok) {
+    // (5) write out: dst[n*ldd + m]
 #pragma unroll
-        for (int i = 0; i < GEMM_NT / 2; i++) {
-            const int n = tile * GEMM_NT + ecol0 + i;
-            if (n < p.N) p.dst[(int64_t)n * p.ldd + m0 + erow] = acc[i];
+    for (int i = 0; i < 16; i++) {
+#pragma unroll
+        for (int c = 0; c < 2; c++) {
+            const int col = gemm_dst_col_t<GROUPED>(p, tile * GEMM_NT + 8 * i + 2 * c4 + c);
+            if (col < 0) continue;
+            if (ok_lo) p.dst[(int64_t)col * p.ldd + m0 + er] = acc[4 * i + c];
+            if (ok_hi) p.dst[(int64_t)col * p.ldd + m0 + er + 8] = acc[4 * i + 2 + c];
         }
     }
-    __syncthreads();
-    if (warp == 0) tmem_dealloc(tmem_base, TM_COLS);
-}
-
-// ================================================================================================ generation 2
-// Same math, same operand images, but the phases of a K block overlap (warp specialisation, the mbarrier pipeline of
-// /opt/skills/guides/blackwell_cuda_programming.md):
-//   warps 0-3  producers : thread r de-quantises row r of the tile, one 64-wide K atom ("step") at a time, into a ring of
-//                          shared-memory stages; thread 0 also starts the bulk copy of the matching activation atom.
-//                          The raw weight bytes of block kb+1 are fetched into registers while block kb is expanded.
-//   warp  8    MMA       : one thread waits for a full stage, issues its tcgen05.mma's, and lets tcgen05.commit hand the
-//                          stage back (empty barrier); after the last step of a K block it commits the accumulator buffer.
-//   warps 4-7  epilogue  : drain the finished accumulator buffer (TMEM is double-buffered by K-block parity, so the MMAs of
-//                          block kb+1 run while block kb is rescaled) with packed fp32x2 FMAs.
-// Steps per K block: Q4_K/Q5_K 4 main atoms + 1 mins atom (stage = A 16 KB + B 16 KB, ring of 6);
-//                    Q6_K      4 atoms, each with the even-scale and the scale-lsb weight tile (A 32 KB + B 16 KB, ring of 4).
-// TMEM: 2 buffers x (main 128 + mins 128) columns = 512 (Q6_K: 2 x 128).
-constexpr int G2_THREADS = 640;                       // warpgroups 0-1 producers, 2-3 epilogue, 4 = MMA warp + 3 idle warps
-constexpr int G2_EPI_WARP0 = 8, G2_MMA_WARP = 16;
-constexpr int G2_ATOM = GEMM_MT * 128;                   // 16 KB: 128 rows x 64 fp16
-
-template <int T>
-struct G2Cfg {
-    static constexpr bool IS_Q6 = (T == T_Q6_K);
-    static constexpr int A_BYTES = IS_Q6 ? 2 * G2_ATOM : G2_ATOM;
-    static constexpr int STAGE_BYTES = A_BYTES + G2_ATOM;
-    static constexpr int NSTAGE = IS_Q6 ? 4 : 6;
-    static constexpr int STEPS = IS_Q6 ? 4 : 5;
-    static constexpr uint32_t TM_COLS = IS_Q6 ? 256 : 512;
-    static constexpr uint32_t TM_BUF = IS_Q6 ? 128 : 256; // columns per accumulator buffer
-    static constexpr size_t SMEM = 1024 + (size_t)NSTAGE * STAGE_BYTES + 256 + 1024;   // + barriers + 2 x 128 activation scales
-};
-
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, uint32_t (&r)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, "
-        "%22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
-// kept in program order (asm volatile) so that the compiler does not hoist all of a block's scale loads above the TMEM loads
-__device__ __forceinline__ float4 ldg_f4_ordered(const float4 * p) {
-    float4 v;
-    asm volatile("ld.global.nc.v4.f32 {%0, %1, %2, %3}, [%4];\n" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "l"(p));
-    return v;
-}
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory"); }
-// The same wait, naming the registers of an earlier tcgen05.ld as in/out operands: their uses cannot be scheduled above the wait even
-// when other work (the math on the previous chunk) sits between the load and the wait.
-__device__ __forceinline__ void tmem_wait_ld(uint32_t (&r)[16]) {
-    asm volatile("tcgen05.wait::ld.sync.aligned;\n"
-                 : "+r"(r[0]), "+r"(r[1]), "+r"(r[2]), "+r"(r[3]), "+r"(r[4]), "+r"(r[5]), "+r"(r[6]), "+r"(r[7]), "+r"(r[8]), "+r"(r[9]), "+r"(r[10]),
-                   "+r"(r[11]), "+r"(r[12]), "+r"(r[13]), "+r"(r[14]), "+r"(r[15])
-                 :: "memory");
-}
-// packed fp32 pairs (sm_100): one issue slot for two FMAs
-__device__ __forceinline__ unsigned long long pk2(float lo, float hi) {
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};\n" : "=l"(r) : "f"(lo), "f"(hi));
-    return r;
-}
-__device__ __forceinline__ unsigned long long pk2u(uint32_t lo, uint32_t hi) {
-    unsigned long long r;
-    asm("mov.b64 %0, {%1, %2};\n" : "=l"(r) : "r"(lo), "r"(hi));
-    return r;
-}
-__device__ __forceinline__ unsigned long long fmul2(unsigned long long a, unsigned long long b) {
-    unsigned long long r;
-    asm("mul.rn.f32x2 %0, %1, %2;\n" : "=l"(r) : "l"(a), "l"(b));
-    return r;
-}
-__device__ __forceinline__ unsigned long long ffma2(unsigned long long a, unsigned long long b, unsigned long long c) {
-    unsigned long long r;
-    asm("fma.rn.f32x2 %0, %1, %2, %3;\n" : "=l"(r) : "l"(a), "l"(b), "l"(c));
-    return r;
-}
-__device__ __forceinline__ void unpk2(unsigned long long v, float & lo, float & hi) { asm("mov.b64 {%0, %1}, %2;\n" : "=f"(lo), "=f"(hi) : "l"(v)); }
-
-// Raw bytes of one weight block, held in registers by the producer thread that owns the row.
-template <int T> struct RawBlock;
-template <> struct RawBlock<T_Q4_K> { uint4 hdr; uint4 qs[8]; };
-template <> struct RawBlock<T_Q5_K> { uint4 hdr; uint4 qh[2]; uint4 qs[8]; };
-template <> struct RawBlock<T_Q6_K> { uint32_t ql[32]; uint32_t qh[16]; uint32_t sc[4]; };
-
-// Producer warpgroup WG (0 / 1) expands steps {0, 1, mins} / {2, 3} of a block (Q6_K: {0, 1} / {2, 3}) and fetches only the
-// bytes those steps read.
-template <int T, int WG>
-__device__ __forceinline__ void g2_load_block(RawBlock<T> & b, const uint8_t * __restrict__ blk, bool valid) {
-    if constexpr (T == T_Q6_K) {
-#pragma unroll
-        for (int i = 0; i < 16; i++) b.ql[16 * WG + i] = valid ? ldg4_a2(blk + 64 * WG + 4 * i) : 0u;
-#pragma unroll
-        for (int i = 0; i < 8; i++) b.qh[8 * WG + i] = valid ? ldg4_a2(blk + 128 + 32 * WG + 4 * i) : 0u;
-#pragma unroll
-        for (int i = 0; i < 2; i++) b.sc[2 * WG + i] = valid ? ldg4_a2(blk + 192 + 8 * WG + 4 * i) : 0u;
-    } else {
-        const uint4 z = make_uint4(0, 0, 0, 0);
-        b.hdr = valid ? __ldg(reinterpret_cast<const uint4 *>(blk)) : z;
-        constexpr int QS_OFF = (T == T_Q4_K) ? 16 : 48;
-        if constexpr (T == T_Q5_K) {
-            b.qh[0] = valid ? __ldg(reinterpret_cast<const uint4 *>(blk + 16)) : z;
-            b.qh[1] = valid ? __ldg(reinterpret_cast<const uint4 *>(blk + 32)) : z;
-        }
-#pragma unroll
-        for (int i = 0; i < 4; i++) b.qs[4 * WG + i] = valid ? __ldg(reinterpret_cast<const uint4 *>(blk + QS_OFF + 16 * (4 * WG + i))) : z;
-    }
-}
-
-// Q4_K / Q5_K, main step g (0..3): weights 64g .. 64g+63 of row r -> one atom.  Low nibbles (sub-block 2g) become
-// (1024+q)*sc - 1024 sc; high nibbles (sub-block 2g+1) are taken in place (value 16 q): (1024+16q)*(sc/16) - 64 sc.  Both are
-// one HFMA2 per pair with a single rounding of an exactly representable result.
-template <int T, int G>
-__device__ __forceinline__ void g2_dequant_main(const RawBlock<T> & b, int r, uint8_t * sA) {
-    int sc0, mn0, sc1, mn1;
-    k4_scale_min(2 * G, b.hdr.y, b.hdr.z, b.hdr.w, sc0, mn0);
-    k4_scale_min(2 * G + 1, b.hdr.y, b.hdr.z, b.hdr.w, sc1, mn1);
-    const __half2 sl = __half2half2(__int2half_rn(sc0)), bl = __half2half2(__int2half_rn(-1024 * sc0));
-    const __half2 sh = __half2half2(__float2half_rn(0.0625f * (float)sc1)), bh = __half2half2(__int2half_rn(-64 * sc1));
-    uint8_t * atom = sA + (r >> 3) * 1024 + (r & 7) * 128;
-#pragma unroll
-    for (int u = 0; u < 2; u++) {
-        const uint4 U = b.qs[2 * G + u];
-        const uint32_t w[4] = {U.x, U.y, U.z, U.w};
-        uint32_t hq[4] = {0, 0, 0, 0};
-        if constexpr (T == T_Q5_K) { const uint4 QH = b.qh[u]; hq[0] = QH.x; hq[1] = QH.y; hq[2] = QH.z; hq[3] = QH.w; }
-#pragma unroll
-        for (int wp = 0; wp < 2; wp++) {
-            uint32_t lo[4], hi[4];
-#pragma unroll
-            for (int i = 0; i < 2; i++) {
-                const uint32_t ww = w[2 * wp + i], ws = ww >> 8;
-                uint32_t l0 = (ww & 0x000F000Fu) | 0x64006400u, l1 = (ws & 0x000F000Fu) | 0x64006400u;
-                uint32_t h0 = (ww & 0x00F000F0u) | 0x64006400u, h1 = (ws & 0x00F000F0u) | 0x64006400u;
-                if constexpr (T == T_Q5_K) {      // 5th bit: bit 2G of qh[l] for low-nibble elements, bit 2G+1 for high-nibble elements
-                    const uint32_t hh = hq[2 * wp + i];
-                    l0 |= ((hh >> (2 * G)) & 0x00010001u) << 4;      l1 |= ((hh >> (2 * G + 8)) & 0x00010001u) << 4;
-                    h0 |= ((hh >> (2 * G + 1)) & 0x00010001u) << 8;  h1 |= ((hh >> (2 * G + 9)) & 0x00010001u) << 8;
-                }
-                lo[2 * i]     = h2_as_u32(__hfma2(*reinterpret_cast<const __half2 *>(&l0), sl, bl));
-                lo[2 * i + 1] = h2_as_u32(__hfma2(*reinterpret_cast<const __half2 *>(&l1), sl, bl));
-                hi[2 * i]     = h2_as_u32(__hfma2(*reinterpret_cast<const __half2 *>(&h0), sh, bh));
-                hi[2 * i + 1] = h2_as_u32(__hfma2(*reinterpret_cast<const __half2 *>(&h1), sh, bh));
-            }
-            const int cl = 2 * u + wp, ch = 4 + 2 * u + wp;
-            *reinterpret_cast<uint4 *>(atom + ((cl ^ (r & 7)) << 4)) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-            *reinterpret_cast<uint4 *>(atom + ((ch ^ (r & 7)) << 4)) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-        }
-    }
-}
-// mins step: kk 0..7 = kk 8..15 = m_j (the activation side holds the even part and the low bit of the sub-block sums)
-template <int T>
-__device__ __forceinline__ void g2_dequant_mins(const RawBlock<T> & b, int r, uint8_t * sA) {
-    uint32_t mh[4];
-#pragma unroll
-    for (int jj = 0; jj < 4; jj++) {
-        int sa, ma, sb, mb;
-        k4_scale_min(2 * jj, b.hdr.y, b.hdr.z, b.hdr.w, sa, ma);
-        k4_scale_min(2 * jj + 1, b.hdr.y, b.hdr.z, b.hdr.w, sb, mb);
-        mh[jj] = h2_as_u32(__halves2half2(__int2half_rn(ma), __int2half_rn(mb)));
-    }
-    uint8_t * arow = sA + (r >> 3) * 1024 + (r & 7) * 128;
-    const uint4 mv = make_uint4(mh[0], mh[1], mh[2], mh[3]);
-    *reinterpret_cast<uint4 *>(arow + ((0 ^ (r & 7)) << 4)) = mv;
-    *reinterpret_cast<uint4 *>(arow + ((1 ^ (r & 7)) << 4)) = mv;
-}
-// Q6_K step A (0..3): weights 64A .. 64A+63 = quarters 2(A&1), 2(A&1)+1 of half A>>1 -> atom of sA1 (even scale part) and sA2 (scale lsb)
-template <int A>
-__device__ __forceinline__ void g2_dequant_q6(const RawBlock<T_Q6_K> & b, int r, uint8_t * sA1, uint8_t * sA2) {
-    constexpr int H = A >> 1;
-    const __half2 k1056 = __half2half2(__int2half_rn(1056));
-    uint8_t * row1 = sA1 + (r >> 3) * 1024 + (r & 7) * 128;
-    uint8_t * row2 = sA2 + (r >> 3) * 1024 + (r & 7) * 128;
-#pragma unroll
-    for (int qq = 0; qq < 2; qq++) {
-        const int qtr = 2 * (A & 1) + qq;
-        __half2 se[2], so[2];
-#pragma unroll
-        for (int hl = 0; hl < 2; hl++) {
-            const int si = 8 * H + 2 * qtr + hl;
-            const int sc = (int)(int8_t)((b.sc[si >> 2] >> (8 * (si & 3))) & 0xFFu);
-            const int lsb = sc & 1;
-            se[hl] = __half2half2(__int2half_rn(sc - lsb));
-            so[hl] = __half2half2(__int2half_rn(lsb));
-        }
-        const int kk0 = 32 * qq;
-#pragma unroll
-        for (int cc = 0; cc < 4; cc++) {
-            uint32_t o1[4], o2[4];
-#pragma unroll
-            for (int i = 0; i < 2; i++) {
-                const int wi = 2 * cc + i;
-                const uint32_t lw = b.ql[16 * H + (qtr & 1) * 8 + wi];
-                const uint32_t hw = b.qh[8 * H + wi];
-                const uint32_t n02 = ((qtr < 2 ? lw : (lw >> 4)) & 0x000F000Fu) | (((hw >> (2 * qtr)) & 0x00030003u) << 4);
-                const uint32_t n13 = ((qtr < 2 ? (lw >> 8) : (lw >> 12)) & 0x000F000Fu) | (((hw >> (2 * qtr + 8)) & 0x00030003u) << 4);
-                const uint32_t m02 = n02 | 0x64006400u, m13 = n13 | 0x64006400u;
-                const __half2 v02 = __hsub2(*reinterpret_cast<const __half2 *>(&m02), k1056);
-                const __half2 v13 = __hsub2(*reinterpret_cast<const __half2 *>(&m13), k1056);
-                const int hl = wi >> 2;
-                o1[2 * i] = h2_as_u32(__hmul2(v02, se[hl])); o1[2 * i + 1] = h2_as_u32(__hmul2(v13, se[hl]));
-                o2[2 * i] = h2_as_u32(__hmul2(v02, so[hl])); o2[2 * i + 1] = h2_as_u32(__hmul2(v13, so[hl]));
-            }
-            const int chunk = (kk0 >> 3) + cc;
-            *reinterpret_cast<uint4 *>(row1 + ((chunk ^ (r & 7)) << 4)) = make_uint4(o1[0], o1[1], o1[2], o1[3]);
-            *reinterpret_cast<uint4 *>(row2 + ((chunk ^ (r & 7)) << 4)) = make_uint4(o2[0], o2[1], o2[2], o2[3]);
-        }
-    }
-}
-
-// One producer warpgroup (128 threads, thread r = row r of the tile): expands its steps of every K block into the stage ring.
-template <int T, int WG>
-__device__ __forceinline__ void g2_producer(const GemmKArgs & p, const uint8_t * wbase, uint8_t * smem, uint64_t * bar_full, uint64_t * bar_empty, int m0, int tile, int nkb, int r) {
-    using C = G2Cfg<T>;
-    constexpr int BB = Fmt<T>::BB;
-    const bool row_ok = m0 + r < p.M;
-    const uint8_t * wrow = wbase + (int64_t)(m0 + r) * p.row_stride;
-    const int64_t bblk = gl::bimg_block_bytes(GEMM_NT);
-    RawBlock<T> cur, nxt;
-    g2_load_block<T, WG>(nxt, wrow, row_ok);
-    for (int kb = 0; kb < nkb; kb++) {
-        cur = nxt;
-        if (kb + 1 < nkb) g2_load_block<T, WG>(nxt, wrow + (int64_t)(kb + 1) * BB, row_ok);
-        const uint8_t * bsrc = p.bimg + ((int64_t)tile * nkb + kb) * bblk;
-#pragma unroll
-        for (int step = 0; step < C::STEPS; step++) {
-            const bool mine = C::IS_Q6 ? ((step >> 1) == WG) : (WG == 0 ? (step < 2 || step == 4) : (step == 2 || step == 3));
-            if (!mine) continue;
-            const uint32_t it = (uint32_t)kb * C::STEPS + step;
-            const uint32_t s = it % C::NSTAGE, ph = (it / C::NSTAGE) & 1u;
-            uint8_t * stA = smem + (size_t)s * C::STAGE_BYTES;
-            g_mbar_wait(bar_empty + s, ph ^ 1u);
-            if (r == 0) {
-                g_mbar_expect_tx(bar_full + s, (uint32_t)G2_ATOM);
-                g_bulk_g2s(stA + C::A_BYTES, bsrc + (int64_t)step * G2_ATOM, (uint32_t)G2_ATOM, bar_full + s);
-            }
-            if constexpr (C::IS_Q6) {
-                if (step == 0) g2_dequant_q6<0>(cur, r, stA, stA + G2_ATOM);
-                else if (step == 1) g2_dequant_q6<1>(cur, r, stA, stA + G2_ATOM);
-                else if (step == 2) g2_dequant_q6<2>(cur, r, stA, stA + G2_ATOM);
-                else g2_dequant_q6<3>(cur, r, stA, stA + G2_ATOM);
-            } else {
-                if (step == 0) g2_dequant_main<T, 0>(cur, r, stA);
-                else if (step == 1) g2_dequant_main<T, 1>(cur, r, stA);
-                else if (step == 2) g2_dequant_main<T, 2>(cur, r, stA);
-                else if (step == 3) g2_dequant_main<T, 3>(cur, r, stA);
-                else g2_dequant_mins<T>(cur, r, stA);
-            }
-            fence_proxy_async();                            // generic-proxy smem writes -> visible to the tensor core (async proxy)
-            g_mbar_arrive(bar_full + s);
-        }
-    }
-}
-
-template <int T, bool GROUPED>
-__global__ void __launch_bounds__(G2_THREADS, 1) gemm_q_tcgen05_v2_kernel(const GemmKArgs p) {
-    // The grouped (MUL_MAT_ID) form is its own instantiation: with the expert lookup and its early exit compiled into the plain GEMM the
-    // kernel went from 44 to 284 bytes of spills (generation 3: 950) and lost a fifth of its throughput.
-    const uint8_t * wbase = p.w;
-    if constexpr (GROUPED) {                               // this column tile's expert (uniform per CTA)
-        const int e = p.tile_expert[blockIdx.y];
-        if (e < 0) return;
-        wbase += (int64_t)e * p.expert_stride;
-    }
-    using C = G2Cfg<T>;
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t * smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t * bars = reinterpret_cast<uint64_t *>(smem + (size_t)C::NSTAGE * C::STAGE_BYTES);
-    uint64_t * bar_full = bars;                            // [NSTAGE] producers (128 arrivals + expect_tx arrival) -> MMA
-    uint64_t * bar_empty = bars + C::NSTAGE;               // [NSTAGE] tcgen05.commit -> producers
-    uint64_t * bar_tfull = bars + 2 * C::NSTAGE;           // [2] tcgen05.commit -> epilogue
-    uint64_t * bar_tempty = bars + 2 * C::NSTAGE + 2;      // [2] epilogue (128 arrivals) -> MMA
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * C::NSTAGE + 4);
-    float * s_da = reinterpret_cast<float *>(smem + (size_t)C::NSTAGE * C::STAGE_BYTES + 256);   // [2][128] d_a of the tile's tokens
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int m0 = blockIdx.x * GEMM_MT, tile = blockIdx.y;
-    const int nkb = p.K >> 8;
-    constexpr int BB = Fmt<T>::BB;
-
-    if (tid == 0) {
-        for (int i = 0; i < C::NSTAGE; i++) { g_mbar_init(bar_full + i, 129); g_mbar_init(bar_empty + i, 1); }
-        for (int i = 0; i < 2; i++) { g_mbar_init(bar_tfull + i, 1); g_mbar_init(bar_tempty + i, 256); }
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    }
-    if (warp == G2_MMA_WARP) tmem_alloc(tmem_slot, C::TM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-
-    // Register file re-split (setmaxnreg is per warpgroup): the epilogue holds a 128 x 128 fp32 tile in registers.
-    // setmaxnreg.inc can only take what the CTA's other warpgroups have RELEASED (the registers the SM had left over at launch
-    // are not in the CTA pool; asking for more spins forever): 640 x 96 at launch; producers 96 -> 80 and the MMA warpgroup
-    // 96 -> 40 release 4096 + 7168 = 11264; the epilogue's 96 -> 136 takes 10240.
-    static_assert(256 * (96 - 80) + 128 * (96 - 40) >= 256 * (136 - 96), "setmaxnreg budget");
-    if (warp < G2_EPI_WARP0) {
-        // ------------------------------------------------------------------ producers (two warpgroups, alternate steps)
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 80;\n");
-        if (warp < 4) g2_producer<T, 0>(p, wbase, smem, bar_full, bar_empty, m0, tile, nkb, tid);
-        else g2_producer<T, 1>(p, wbase, smem, bar_full, bar_empty, m0, tile, nkb, tid - 128);
-    } else if (warp >= G2_MMA_WARP) {
-        // ------------------------------------------------------------------ MMA issuer (one warp; its 3 warpgroup mates only give their registers away)
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n");
-        if (warp == G2_MMA_WARP) {
-        const uint32_t idesc = make_idesc_f16(GEMM_MT, GEMM_NT);
-        uint32_t it = 0;
-        for (int kb = 0; kb < nkb; kb++) {
-            const uint32_t buf = (uint32_t)kb & 1u, use = (uint32_t)kb >> 1;
-            g_mbar_wait(bar_tempty + buf, (use & 1u) ^ 1u);
-            tc_fence_after();
-            const uint32_t t_main = tmem_base + buf * C::TM_BUF, t_mins = t_main + GEMM_NT;
-#pragma unroll
-            for (int step = 0; step < C::STEPS; step++, it++) {
-                const uint32_t s = it % C::NSTAGE, ph = (it / C::NSTAGE) & 1u;
-                g_mbar_wait(bar_full + s, ph);
-                tc_fence_after();
-                if (lane == 0) {
-                    const uint32_t aA = s32(smem + (size_t)s * C::STAGE_BYTES), aB = aA + C::A_BYTES;
-                    if constexpr (C::IS_Q6) {
-#pragma unroll
-                        for (int ks = 0; ks < 4; ks++) {
-                            umma_f16(t_main, make_desc_sw128(aA + ks * 32), make_desc_sw128(aB + ks * 32), idesc, (step | ks) != 0 ? 1u : 0u);
-                            umma_f16(t_main, make_desc_sw128(aA + G2_ATOM + ks * 32), make_desc_sw128(aB + ks * 32), idesc, 1u);
-                        }
-                    } else {
-                        if (step < 4) {
-#pragma unroll
-                            for (int ks = 0; ks < 4; ks++)
-                                umma_f16(t_main, make_desc_sw128(aA + ks * 32), make_desc_sw128(aB + ks * 32), idesc, (step | ks) != 0 ? 1u : 0u);
-                        } else {
-                            umma_f16(t_mins, make_desc_sw128(aA), make_desc_sw128(aB), idesc, 0u);
-                        }
-                    }
-                    umma_commit(bar_empty + s);             // the stage is free once these MMAs have read it
-                    if (step == C::STEPS - 1) umma_commit(bar_tfull + buf);
-                }
-                __syncwarp();
-            }
-        }
-        }
-    } else {
-        // ------------------------------------------------------------------ epilogue (8 warps: TMEM lanes 32 (warp & 3) .., column half (warp - 8) >> 2)
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 136;\n");
-        const int q4 = warp & 3, chalf = (warp - G2_EPI_WARP0) >> 2;
-        constexpr int ECOLS = GEMM_NT / 2;
-        const int erow = 32 * q4 + lane;
-        const bool erow_ok = m0 + erow < p.M;
-        const uint8_t * ewrow = wbase + (int64_t)(m0 + erow) * p.row_stride;
-        unsigned long long acc[ECOLS / 2];
-#pragma unroll
-        for (int i = 0; i < ECOLS / 2; i++) acc[i] = 0ull;
-        const int et = tid - 32 * G2_EPI_WARP0;             // 0..255
-        const float * dag = p.da + tile * GEMM_NT + (et & 127);
-        if (et < GEMM_NT) s_da[et] = __ldg(dag);
-        asm volatile("bar.sync 1, 256;\n" ::: "memory");
-        for (int kb = 0; kb < nkb; kb++) {
-            const uint32_t buf = (uint32_t)kb & 1u, use = (uint32_t)kb >> 1;
-            if (kb + 1 < nkb && et < GEMM_NT) s_da[((kb + 1) & 1) * GEMM_NT + et] = __ldg(dag + (int64_t)(kb + 1) * p.npad);
-            float dw = 0.0f, dm = 0.0f;
-            if (erow_ok) {
-                if constexpr (C::IS_Q6) {
-                    dw = __half2float(__ushort_as_half(__ldg(reinterpret_cast<const unsigned short *>(ewrow + (int64_t)kb * BB + 208))));
-                } else {
-                    const uint32_t dd = __ldg(reinterpret_cast<const uint32_t *>(ewrow + (int64_t)kb * BB));
-                    dw = __half2float(__ushort_as_half((unsigned short)(dd & 0xFFFFu)));
-                    dm = __half2float(__ushort_as_half((unsigned short)(dd >> 16)));
-                }
-            }
-            const unsigned long long dw2 = pk2(dw, dw), ndm2 = pk2(-dm, -dm);
-            const float4 * dap = reinterpret_cast<const float4 *>(s_da + (kb & 1) * GEMM_NT + chalf * ECOLS);
-            g_mbar_wait(bar_tfull + buf, use & 1u);
-            tc_fence_after();
-            const uint32_t tlane = tmem_base + buf * C::TM_BUF + ((uint32_t)(32 * q4) << 16) + (uint32_t)(chalf * ECOLS);
-#pragma unroll
-            for (int c = 0; c < ECOLS; c += 16) {
-                uint32_t vm[16], vn[16];
-                tmem_ld16_nowait(tlane + (uint32_t)c, vm);
-                if constexpr (!C::IS_Q6) tmem_ld16_nowait(tlane + (uint32_t)(GEMM_NT + c), vn);
-                tmem_wait_ld();
-                if (c + 16 == ECOLS) {                      // everything of this buffer is in registers: hand it back to the MMA warp
-                    tc_fence_before();
-                    g_mbar_arrive(bar_tempty + buf);
-                }
-#pragma unroll
-                for (int i = 0; i < 16; i += 4) {
-                    const float4 da = dap[(c + i) >> 2];
-                    const unsigned long long da01 = pk2(da.x, da.y), da23 = pk2(da.z, da.w);
-                    unsigned long long t0 = fmul2(dw2, pk2u(vm[i], vm[i + 1])), t1 = fmul2(dw2, pk2u(vm[i + 2], vm[i + 3]));
-                    if constexpr (!C::IS_Q6) {
-                        t0 = ffma2(ndm2, pk2u(vn[i], vn[i + 1]), t0);
-                        t1 = ffma2(ndm2, pk2u(vn[i + 2], vn[i + 3]), t1);
-                    }
-                    acc[(c + i) >> 1] = ffma2(da01, t0, acc[(c + i) >> 1]);
-                    acc[((c + i) >> 1) + 1] = ffma2(da23, t1, acc[((c + i) >> 1) + 1]);
-                }
-            }
-            asm volatile("bar.sync 1, 256;\n" ::: "memory");   // s_da[kb & 1] fully read, s_da[(kb + 1) & 1] written
-        }
-        if (erow_ok) {
-#pragma unroll
-            for (int i = 0; i < ECOLS / 2; i++) {
-                float lo, hi;
-                unpk2(acc[i], lo, hi);
-                const int n = tile * GEMM_NT + chalf * ECOLS + 2 * i;
-                const int c0 = gemm_dst_col_t<GROUPED>(p, n), c1 = gemm_dst_col_t<GROUPED>(p, n + 1);
-                if (c0 >= 0) p.dst[(int64_t)c0 * p.ldd + m0 + erow] = lo;
-                if (c1 >= 0) p.dst[(int64_t)c1 * p.ldd + m0 + erow] = hi;
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == G2_MMA_WARP) { tc_fence_after(); tmem_dealloc(tmem_base, C::TM_COLS); }
-}
-
-
-// ================================================================================================ generation 3 (Q4_K / Q5_K)
-// What limited generation 2 (ncu, profiles/r01_gemm_v2_ncu.md, and the issue-slot count in DESIGN.md 5.1): per 256-weight K block a
-// 128 x 128 tile is 1 050 cycles of MMA, but the CUDA cores have to issue ~2 000 warp instructions to de-quantise the 128 x 256
-// weights and ~2 800 to drain and rescale 2 x 128 x 128 accumulators -- 4.6 instructions per cycle on an SM that issues 4.  The
-// de-quantised A tile is the expensive operand, so generation 3 uses it for MORE token columns:
-//   * tile 128 x 192: one A tile feeds 192 columns (1.5x the MMA work per de-quantised weight); 5 stages of A 16 KB + B 24 KB;
-//   * TMEM: main 192 + mins 192 columns, SINGLE-buffered, but pipelined in two ways: the mins MMA (one K=16 instruction) is issued
-//     FIRST in a block, so its accumulator drains while the 16 main MMAs run; and the main accumulator is split in two halves of
-//     96 columns with their own full/empty barriers, drained by one epilogue warpgroup each -- the MMAs of the next block start on
-//     half 0 as soon as half 0 is in registers;
-//   * 14336 x 2048: 112 x 11 tiles = 8.3 waves of 148 CTAs instead of 12.1.
-// Arithmetic is unchanged (exact-integer operands, per-block fp32 combine); only the order of the two fp32 updates of a block
-// differs (mins term first).
-constexpr int G3_HALF   = GEMM_NT3 / 2;                   // 96 columns per accumulator half
-constexpr int G3_BATOM  = GEMM_NT3 * 128;                 // 24 KB: 192 token rows x 64 fp16
-constexpr int G3_STAGE  = G2_ATOM + G3_BATOM;             // 40 KB
-constexpr int G3_NSTAGE = 5;
-constexpr int G3_STEPS  = 5;                              // mins, main 0..3
-constexpr uint32_t G3_TM_COLS = 512;                      // power of two >= 384
-constexpr size_t G3_SMEM = 1024 + (size_t)G3_NSTAGE * G3_STAGE + 256 + 2 * GEMM_NT3 * 4 + 64;
-
-template <int T, int WG>
-__device__ __forceinline__ void g3_producer(const GemmKArgs & p, const uint8_t * wbase, uint8_t * smem, uint64_t * bar_full, uint64_t * bar_empty, int m0, int tile, int nkb, int r) {
-    constexpr int BB = Fmt<T>::BB;
-    const bool row_ok = m0 + r < p.M;
-    const uint8_t * wrow = wbase + (int64_t)(m0 + r) * p.row_stride;
-    const int64_t bblk = gl::bimg_block_bytes(GEMM_NT3);
-    RawBlock<T> cur, nxt;
-    g2_load_block<T, WG>(nxt, wrow, row_ok);
-    for (int kb = 0; kb < nkb; kb++) {
-        cur = nxt;
-        if (kb + 1 < nkb) g2_load_block<T, WG>(nxt, wrow + (int64_t)(kb + 1) * BB, row_ok);
-        const uint8_t * bsrc = p.bimg + ((int64_t)tile * nkb + kb) * bblk;
-#pragma unroll
-        for (int step = 0; step < G3_STEPS; step++) {             // step 0: mins; step g + 1: weights 64g .. 64g + 63
-            const bool mine = WG == 0 ? step <= 2 : step >= 3;
-            if (!mine) continue;
-            const uint32_t it = (uint32_t)kb * G3_STEPS + step;
-            const uint32_t s = it % G3_NSTAGE, ph = (it / G3_NSTAGE) & 1u;
-            uint8_t * stA = smem + (size_t)s * G3_STAGE;
-            g_mbar_wait(bar_empty + s, ph ^ 1u);
-            if (r == 0) {
-                g_mbar_expect_tx(bar_full + s, (uint32_t)G3_BATOM);
-                g_bulk_g2s(stA + G2_ATOM, bsrc + (int64_t)(step == 0 ? 4 : step - 1) * G3_BATOM, (uint32_t)G3_BATOM, bar_full + s);
-            }
-            if (step == 0) g2_dequant_mins<T>(cur, r, stA);
-            else if (step == 1) g2_dequant_main<T, 0>(cur, r, stA);
-            else if (step == 2) g2_dequant_main<T, 1>(cur, r, stA);
-            else if (step == 3) g2_dequant_main<T, 2>(cur, r, stA);
-            else g2_dequant_main<T, 3>(cur, r, stA);
-            fence_proxy_async();
-            g_mbar_arrive(bar_full + s);
-        }
-    }
-}
-
-template <int T, bool GROUPED>
-__global__ void __launch_bounds__(G2_THREADS, 1) gemm_q_tcgen05_v3_kernel(const GemmKArgs p) {
-    // The grouped (MUL_MAT_ID) form is its own instantiation: with the expert lookup and its early exit compiled into the plain GEMM the
-    // kernel went from 44 to 284 bytes of spills (generation 3: 950) and lost a fifth of its throughput.
-    const uint8_t * wbase = p.w;
-    if constexpr (GROUPED) {                               // this column tile's expert (uniform per CTA)
-        const int e = p.tile_expert[blockIdx.y];
-        if (e < 0) return;
-        wbase += (int64_t)e * p.expert_stride;
-    }
-    static_assert(T == T_Q4_K || T == T_Q5_K, "generation 3 covers the formats with a mins term");
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t * smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    uint64_t * bars = reinterpret_cast<uint64_t *>(smem + (size_t)G3_NSTAGE * G3_STAGE);
-    uint64_t * bar_full = bars;                            // [5] producers (128 arrivals + expect_tx arrival) -> MMA
-    uint64_t * bar_empty = bars + G3_NSTAGE;               // [5] tcgen05.commit -> producers
-    uint64_t * bar_mins_full = bars + 2 * G3_NSTAGE;       // tcgen05.commit -> epilogue
-    uint64_t * bar_mins_empty = bar_mins_full + 1;         // epilogue (256 arrivals) -> MMA
-    uint64_t * bar_main_full = bar_mins_full + 2;          // [2] per accumulator half
-    uint64_t * bar_main_empty = bar_mins_full + 4;         // [2] 128 arrivals each
-    uint32_t * tmem_slot = reinterpret_cast<uint32_t *>(bar_mins_full + 6);
-    float * s_da = reinterpret_cast<float *>(smem + (size_t)G3_NSTAGE * G3_STAGE + 256);   // [2][192] d_a of the tile's tokens
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int m0 = blockIdx.x * GEMM_MT, tile = blockIdx.y;
-    const int nkb = p.K >> 8;
-    constexpr int BB = Fmt<T>::BB;
-
-    if (tid == 0) {
-        for (int i = 0; i < G3_NSTAGE; i++) { g_mbar_init(bar_full + i, 129); g_mbar_init(bar_empty + i, 1); }
-        g_mbar_init(bar_mins_full, 1); g_mbar_init(bar_mins_empty, 256);
-        for (int i = 0; i < 2; i++) { g_mbar_init(bar_main_full + i, 1); g_mbar_init(bar_main_empty + i, 128); }
-        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
-    }
-    if (warp == G2_MMA_WARP) tmem_alloc(tmem_slot, G3_TM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t t_main = tmem_base, t_mins = tmem_base + GEMM_NT3;
-
-    static_assert(256 * (96 - 72) + 128 * (96 - 24) >= 256 * (152 - 96), "setmaxnreg budget");
-    if (warp < G2_EPI_WARP0) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 72;\n");
-        if (warp < 4) g3_producer<T, 0>(p, wbase, smem, bar_full, bar_empty, m0, tile, nkb, tid);
-        else g3_producer<T, 1>(p, wbase, smem, bar_full, bar_empty, m0, tile, nkb, tid - 128);
-    } else if (warp >= G2_MMA_WARP) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 24;\n");
-        if (warp == G2_MMA_WARP) {
-            const uint32_t idesc_half = make_idesc_f16(GEMM_MT, G3_HALF), idesc_mins = make_idesc_f16(GEMM_MT, GEMM_NT3);
-            uint32_t it = 0;
-            for (int kb = 0; kb < nkb; kb++) {
-                const uint32_t par = (uint32_t)kb & 1u;
-                // ---- mins: one K = 16 MMA over all 192 columns, first in the block (its accumulator drains under the main MMAs)
-                g_mbar_wait(bar_mins_empty, par ^ 1u);
-                {
-                    const uint32_t s = it % G3_NSTAGE, ph = (it / G3_NSTAGE) & 1u;
-                    g_mbar_wait(bar_full + s, ph);
-                    tc_fence_after();
-                    if (lane == 0) {
-                        const uint32_t aA = s32(smem + (size_t)s * G3_STAGE), aB = aA + G2_ATOM;
-                        umma_f16(t_mins, make_desc_sw128(aA), make_desc_sw128(aB), idesc_mins, 0u);
-                        umma_commit(bar_empty + s);
-                        umma_commit(bar_mins_full);
-                    }
-                    __syncwarp();
-                    it++;
-                }
-                // ---- main: 4 steps x (4 MMAs into half 0, 4 into half 1)
-#pragma unroll
-                for (int g = 0; g < 4; g++, it++) {
-                    const uint32_t s = it % G3_NSTAGE, ph = (it / G3_NSTAGE) & 1u;
-                    g_mbar_wait(bar_full + s, ph);
-                    const uint32_t aA = s32(smem + (size_t)s * G3_STAGE), aB = aA + G2_ATOM;
-#pragma unroll
-                    for (int h = 0; h < 2; h++) {
-                        if (g == 0) g_mbar_wait(bar_main_empty + h, par ^ 1u);       // half h of the previous block is in registers
-                        tc_fence_after();
-                        if (lane == 0) {
-#pragma unroll
-                            for (int ks = 0; ks < 4; ks++)
-                                umma_f16(t_main + (uint32_t)(h * G3_HALF), make_desc_sw128(aA + ks * 32), make_desc_sw128(aB + h * G3_HALF * 128 + ks * 32), idesc_half,
-                                         (g | ks) != 0 ? 1u : 0u);
-                            if (g == 3) umma_commit(bar_main_full + h);
-                            if (h == 1) umma_commit(bar_empty + s);
-                        }
-                        __syncwarp();
-                    }
-                }
-            }
-        }
-    } else {
-        // ------------------------------------------------------------------ epilogue: warpgroup e drains half e (TMEM lanes 32 (warp & 3) ..)
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 152;\n");
-        const int q4 = warp & 3, half = (warp - G2_EPI_WARP0) >> 2;
-        const int erow = 32 * q4 + lane;
-        const bool erow_ok = m0 + erow < p.M;
-        const uint8_t * ewrow = wbase + (int64_t)(m0 + erow) * p.row_stride;
-        unsigned long long acc[G3_HALF / 2];
-#pragma unroll
-        for (int i = 0; i < G3_HALF / 2; i++) acc[i] = 0ull;
-        const int et = tid - 32 * G2_EPI_WARP0;             // 0..255
-        const float * dag = p.da + tile * GEMM_NT3 + et;
-        if (et < GEMM_NT3) s_da[et] = __ldg(dag);
-        asm volatile("bar.sync 1, 256;\n" ::: "memory");
-        const uint32_t tlane = tmem_base + ((uint32_t)(32 * q4) << 16) + (uint32_t)(half * G3_HALF);
-        for (int kb = 0; kb < nkb; kb++) {
-            const uint32_t par = (uint32_t)kb & 1u;
-            if (kb + 1 < nkb && et < GEMM_NT3) s_da[((kb + 1) & 1) * GEMM_NT3 + et] = __ldg(dag + (int64_t)(kb + 1) * p.npad);
-            float dw = 0.0f, dm = 0.0f;
-            if (erow_ok) {
-                const uint32_t dd = __ldg(reinterpret_cast<const uint32_t *>(ewrow + (int64_t)kb * BB));
-                dw = __half2float(__ushort_as_half((unsigned short)(dd & 0xFFFFu)));
-                dm = __half2float(__ushort_as_half((unsigned short)(dd >> 16)));
-            }
-            const unsigned long long dw2 = pk2(dw, dw), ndm2 = pk2(-dm, -dm);
-            const float4 * dap = reinterpret_cast<const float4 *>(s_da + (kb & 1) * GEMM_NT3 + half * G3_HALF);
-            // One accumulator half = 6 chunks of 16 columns.  A tcgen05.ld takes several hundred cycles under the MMA's own TMEM traffic
-            // and tcgen05.wait::ld waits for ALL outstanding loads, so the chunks are software-pipelined one deep: chunk i + 1 is in
-            // flight while chunk i is scaled and accumulated (the first version loaded, waited and computed strictly in turn: 12 exposed
-            // load latencies per K block, ~7 700 cycles against ~1 600 of MMA).
-            auto drain_half = [&](uint32_t taddr, unsigned long long scale2, uint64_t * bar_release) {
-                uint32_t v0[16], v1[16];
-                auto fma_chunk = [&](int c, const uint32_t (&v)[16]) {
-#pragma unroll
-                    for (int i = 0; i < 16; i += 4) {
-                        const float4 da = dap[(c + i) >> 2];
-                        acc[(c + i) >> 1] = ffma2(pk2(da.x, da.y), fmul2(scale2, pk2u(v[i], v[i + 1])), acc[(c + i) >> 1]);
-                        acc[((c + i) >> 1) + 1] = ffma2(pk2(da.z, da.w), fmul2(scale2, pk2u(v[i + 2], v[i + 3])), acc[((c + i) >> 1) + 1]);
-                    }
-                };
-                tmem_ld16_nowait(taddr, v0);
-                tmem_wait_ld(v0);
-#pragma unroll
-                for (int c = 0; c < G3_HALF; c += 32) {
-                    tmem_ld16_nowait(taddr + (uint32_t)(c + 16), v1);
-                    fma_chunk(c, v0);
-                    tmem_wait_ld(v1);
-                    if (c + 32 < G3_HALF) tmem_ld16_nowait(taddr + (uint32_t)(c + 32), v0);
-                    else { tc_fence_before(); g_mbar_arrive(bar_release); }       // this half's TMEM columns are in registers
-                    fma_chunk(c + 16, v1);
-                    if (c + 32 < G3_HALF) tmem_wait_ld(v0);
-                }
-            };
-            // ---- mins term: acc += d_a * (-dmin_w * mins)
-            g_mbar_wait(bar_mins_full, par);
-            tc_fence_after();
-            drain_half(tlane + (uint32_t)GEMM_NT3, ndm2, bar_mins_empty);
-            // ---- main term: acc += d_a * (d_w * main)
-            g_mbar_wait(bar_main_full + half, par);
-            tc_fence_after();
-            drain_half(tlane, dw2, bar_main_empty + half);
-            asm volatile("bar.sync 1, 256;\n" ::: "memory");   // s_da[kb & 1] fully read, s_da[(kb + 1) & 1] written
-        }
-        if (erow_ok) {
-#pragma unroll
-            for (int i = 0; i < G3_HALF / 2; i++) {
-                float lo, hi;
-                unpk2(acc[i], lo, hi);
-                const int n = tile * GEMM_NT3 + half * G3_HALF + 2 * i;
-                const int c0 = gemm_dst_col_t<GROUPED>(p, n), c1 = gemm_dst_col_t<GROUPED>(p, n + 1);
-                if (c0 >= 0) p.dst[(int64_t)c0 * p.ldd + m0 + erow] = lo;
-                if (c1 >= 0) p.dst[(int64_t)c1 * p.ldd + m0 + erow] = hi;
-            }
-        }
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == G2_MMA_WARP) { tc_fence_after(); tmem_dealloc(tmem_base, G3_TM_COLS); }
 }
 
 template <int T>
-static cudaError_t launch_v3(const GemmKArgs & k, dim3 grid, cudaStream_t st) {
+static cudaError_t launch_kq(const GemmKArgs & k, dim3 grid, cudaStream_t st) {
     static bool attr_done[64] = {};
     int dev = 0;
     cudaGetDevice(&dev);
     dev &= 63;
     if (!attr_done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_q_tcgen05_v3_kernel<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G3_SMEM);
+        cudaError_t e = cudaFuncSetAttribute(gemm_q_wgmma_kernel<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)KqCfg<T>::SMEM);
         if (e != cudaSuccess) return e;
-        e = cudaFuncSetAttribute(gemm_q_tcgen05_v3_kernel<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G3_SMEM);
+        e = cudaFuncSetAttribute(gemm_q_wgmma_kernel<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)KqCfg<T>::SMEM);
         if (e != cudaSuccess) return e;
         attr_done[dev] = true;
     }
-    if (k.tile_expert != nullptr) gemm_q_tcgen05_v3_kernel<T, true><<<grid, G2_THREADS, G3_SMEM, st>>>(k);
-    else gemm_q_tcgen05_v3_kernel<T, false><<<grid, G2_THREADS, G3_SMEM, st>>>(k);
+    if (k.tile_expert != nullptr) gemm_q_wgmma_kernel<T, true><<<grid, GEMM_THREADS, KqCfg<T>::SMEM, st>>>(k);
+    else gemm_q_wgmma_kernel<T, false><<<grid, GEMM_THREADS, KqCfg<T>::SMEM, st>>>(k);
     return cudaGetLastError();
 }
-
-static int g_gemm_variant = [] { const char * e = getenv("GGML_B200_GEMM_VARIANT"); return (e && e[0] >= '1' && e[0] <= '3') ? e[0] - '0' : 2; }();
-void set_gemm_variant(int v) { g_gemm_variant = (v >= 1 && v <= 3) ? v : 2; }
 
 // which operand images the workspace holds (0 K-quant, 1 legacy): a caller's reuse_operands flag only names the activation
 static thread_local int g_last_gemm_family = 0;
 static thread_local bool g_kquant_images_stale = false;
 static inline void g_last_gemm_family_guard() { if (g_last_gemm_family == 1) { g_kquant_images_stale = true; g_last_gemm_family = 0; } }
-
-template <int T>
-static cudaError_t launch_v2(const GemmKArgs & k, dim3 grid, cudaStream_t st) {
-    static bool attr_done[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    dev &= 63;
-    if (!attr_done[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(gemm_q_tcgen05_v2_kernel<T, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G2Cfg<T>::SMEM);
-        if (e != cudaSuccess) return e;
-        e = cudaFuncSetAttribute(gemm_q_tcgen05_v2_kernel<T, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)G2Cfg<T>::SMEM);
-        if (e != cudaSuccess) return e;
-        attr_done[dev] = true;
-    }
-    if (k.tile_expert != nullptr) gemm_q_tcgen05_v2_kernel<T, true><<<grid, G2_THREADS, G2Cfg<T>::SMEM, st>>>(k);
-    else gemm_q_tcgen05_v2_kernel<T, false><<<grid, G2_THREADS, G2Cfg<T>::SMEM, st>>>(k);
-    return cudaGetLastError();
-}
 
 cudaError_t launch_gemm(int type, const GemmArgs & a, cudaStream_t st) {
     if (type == T_Q4_0 || type == T_Q8_0) {
@@ -1097,66 +427,36 @@ cudaError_t launch_gemm(int type, const GemmArgs & a, cudaStream_t st) {
     g_last_gemm_family_guard();
     if (!(type == T_Q4_K || type == T_Q5_K || type == T_Q6_K) || a.K % 256 || a.N <= 0 || a.M <= 0) return cudaErrorNotSupported;
     if (type == T_Q6_K ? ((reinterpret_cast<uintptr_t>(a.w) & 1) || (a.row_stride & 1)) : ((reinterpret_cast<uintptr_t>(a.w) & 15) || (a.row_stride & 15))) return cudaErrorMisalignedAddress;
-    const bool gen3 = g_gemm_variant == 3 && type != T_Q6_K;
-    const int NT = gen3 ? GEMM_NT3 : GEMM_NT;
+    const int NT = GEMM_NT;
     const int npad = (int)rup(a.N, NT), nkb = a.K / 256, ntiles = npad / NT;
     if (a.workspace_bytes < gemm_workspace_bytes(type, a.M, a.N, a.K)) return cudaErrorInvalidValue;
     if ((reinterpret_cast<uintptr_t>(a.x) & 15) || (a.ldx & 3)) return cudaErrorMisalignedAddress;   // the pre-pass reads float4
     uint8_t * bimg = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(a.workspace) + 255) & ~uintptr_t(255));
     float * da = reinterpret_cast<float *>(bimg + (int64_t)ntiles * nkb * gl::bimg_block_bytes(NT));
     cudaError_t e = cudaSuccess;
-    // the operand images in the workspace are laid out for one tile width: a caller's "same activation as last time" only holds if the
-    // previous launch on this workspace used the same width
     static thread_local const void * last_ws = nullptr;
-    static thread_local int last_nt = 0;
-    const bool reuse = a.reuse_operands && last_ws == a.workspace && last_nt == NT && !g_kquant_images_stale;
+    const bool reuse = a.reuse_operands && last_ws == a.workspace && !g_kquant_images_stale;
     g_kquant_images_stale = false;
-    last_ws = a.workspace; last_nt = NT;
+    last_ws = a.workspace;
     if (!reuse) {
         note_launch();
         quantize_act_gemm_kernel<<<dim3((unsigned)nkb, (unsigned)(npad / 8)), 256, 0, st>>>(a.x, a.ldx, a.N, nkb, npad, bimg, da, NT, nullptr);
         e = cudaGetLastError();
         if (e != cudaSuccess) return e;
     }
-
-    constexpr size_t SMEM = 1024 + 5 * (GEMM_MT * 128) + 5 * (GEMM_NT * 128) + GEMM_NT * 4 + 64;
-    constexpr size_t SMEM6 = 1024 + 8 * (GEMM_MT * 128) + 5 * (GEMM_NT * 128) + GEMM_NT * 4 + 64;
-    static bool attr_done[64] = {};
-    int dev = 0;
-    cudaGetDevice(&dev);
-    dev &= 63;
-    if (!attr_done[dev]) {
-        e = cudaFuncSetAttribute(gemm_q_tcgen05_kernel<T_Q4_K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
-        if (e != cudaSuccess) return e;
-        e = cudaFuncSetAttribute(gemm_q_tcgen05_kernel<T_Q5_K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM);
-        if (e != cudaSuccess) return e;
-        e = cudaFuncSetAttribute(gemm_q_tcgen05_kernel<T_Q6_K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SMEM6);
-        if (e != cudaSuccess) return e;
-        attr_done[dev] = true;
-    }
     GemmKArgs k{a.w, a.row_stride, a.M, a.K, a.N, npad, bimg, da, a.dst, a.ldd, nullptr, nullptr, 0};
     const dim3 grid((unsigned)((a.M + GEMM_MT - 1) / GEMM_MT), (unsigned)ntiles);
     note_launch();
-    if (gen3) {
-        if (type == T_Q4_K) return launch_v3<T_Q4_K>(k, grid, st);
-        return launch_v3<T_Q5_K>(k, grid, st);
-    }
-    if (g_gemm_variant >= 2) {
-        if (type == T_Q4_K) return launch_v2<T_Q4_K>(k, grid, st);
-        if (type == T_Q5_K) return launch_v2<T_Q5_K>(k, grid, st);
-        return launch_v2<T_Q6_K>(k, grid, st);
-    }
-    if (type == T_Q4_K) gemm_q_tcgen05_kernel<T_Q4_K><<<grid, GEMM_THREADS, SMEM, st>>>(k);
-    else if (type == T_Q5_K) gemm_q_tcgen05_kernel<T_Q5_K><<<grid, GEMM_THREADS, SMEM, st>>>(k);
-    else gemm_q_tcgen05_kernel<T_Q6_K><<<grid, GEMM_THREADS, SMEM6, st>>>(k);
-    return cudaGetLastError();
+    if (type == T_Q4_K) return launch_kq<T_Q4_K>(k, grid, st);
+    if (type == T_Q5_K) return launch_kq<T_Q5_K>(k, grid, st);
+    return launch_kq<T_Q6_K>(k, grid, st);
 }
 
 // ------------------------------------------------------------------------------------------------ grouped GEMM (MUL_MAT_ID, many tokens)
 // ggml_compute_forward_mul_mat_id (ggml-cpu.c:1534-1707) groups the (token, slot) rows by expert on one thread and runs one mat-mul
 // per expert.  Here: one small kernel sorts the jobs by expert into column tiles (all on the device, no host round trip: the launch
 // covers the worst-case number of tiles and the tiles that do not exist exit at once), the activation pre-pass gathers each tile's
-// columns, and the tcgen05 kernels take the expert's weights per tile and scatter the output columns.
+// columns, and the GEMM kernel takes the expert's weights per tile and scatters the output columns.
 __global__ void __launch_bounds__(1024) moe_route_kernel(const int32_t * __restrict__ ids, int64_t ids_stride, int T, int n_used, int nb1, int n_expert, int NT, int max_tiles,
                                                          int * __restrict__ tile_expert, int * __restrict__ col_src, int * __restrict__ col_dst) {
     __shared__ int cnt[256], base[256], fill[256];
@@ -1192,7 +492,7 @@ __global__ void __launch_bounds__(1024) moe_route_kernel(const int32_t * __restr
 size_t gemm_grouped_workspace_bytes(int type, int64_t M, int64_t jobs, int64_t n_expert, int64_t K) {
     (void)M;
     if (!(type == T_Q4_K || type == T_Q5_K || type == T_Q6_K) || K % 256 || jobs <= 0 || n_expert > 256) return 0;
-    const int NT = type == T_Q6_K ? GEMM_NT : GEMM_NT3;
+    const int NT = GEMM_NT;
     const int64_t max_tiles = (jobs + NT - 1) / NT + n_expert, nkb = K / 256;
     return (size_t)(max_tiles * nkb * gl::bimg_block_bytes(NT) + nkb * max_tiles * NT * 4 + (max_tiles + 2 * max_tiles * NT) * 4 + 2048);
 }
@@ -1201,8 +501,7 @@ cudaError_t launch_gemm_grouped(int type, const GemmGroupedArgs & a, cudaStream_
     if (!(type == T_Q4_K || type == T_Q5_K || type == T_Q6_K) || a.K % 256 || a.M <= 0 || a.T <= 0 || a.n_used <= 0 || a.n_expert <= 0 || a.n_expert > 256) return cudaErrorNotSupported;
     if (type == T_Q6_K ? ((reinterpret_cast<uintptr_t>(a.w) & 1) || (a.row_stride & 1) || (a.expert_stride & 1)) : ((reinterpret_cast<uintptr_t>(a.w) & 15) || (a.row_stride & 15) || (a.expert_stride & 15))) return cudaErrorMisalignedAddress;
     if ((reinterpret_cast<uintptr_t>(a.x) & 15) || (a.ldx & 3)) return cudaErrorMisalignedAddress;
-    const bool gen3 = type != T_Q6_K;
-    const int NT = gen3 ? GEMM_NT3 : GEMM_NT;
+    const int NT = GEMM_NT;
     const int64_t jobs = (int64_t)a.T * a.n_used;
     const int max_tiles = (int)((jobs + NT - 1) / NT + a.n_expert), nkb = a.K / 256, npad = max_tiles * NT;
     if (a.workspace_bytes < gemm_grouped_workspace_bytes(type, a.M, jobs, a.n_expert, a.K)) return cudaErrorInvalidValue;
@@ -1220,9 +519,9 @@ cudaError_t launch_gemm_grouped(int type, const GemmGroupedArgs & a, cudaStream_
     GemmKArgs k{a.w, a.row_stride, a.M, a.K, npad, npad, bimg, da, a.dst, a.ldd, tile_expert, col_dst, a.expert_stride};
     const dim3 grid((unsigned)((a.M + GEMM_MT - 1) / GEMM_MT), (unsigned)max_tiles);
     note_launch();
-    if (type == T_Q4_K) return launch_v3<T_Q4_K>(k, grid, st);
-    if (type == T_Q5_K) return launch_v3<T_Q5_K>(k, grid, st);
-    return launch_v2<T_Q6_K>(k, grid, st);
+    if (type == T_Q4_K) return launch_kq<T_Q4_K>(k, grid, st);
+    if (type == T_Q5_K) return launch_kq<T_Q5_K>(k, grid, st);
+    return launch_kq<T_Q6_K>(k, grid, st);
 }
 
 }  // namespace qmm

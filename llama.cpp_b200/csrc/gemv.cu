@@ -1,4 +1,4 @@
-// gemv.cu -- decode mat-vec for GGUF block formats on sm_100a:  dst[M, n] = W[M, K] . act[K, n],  n <= 8.
+// gemv.cu -- decode mat-vec for GGUF block formats on sm_90a:  dst[M, n] = W[M, K] . act[K, n],  n <= 8.
 //
 // Replaces, for the batch-1 regime, the inner loop of ggml_compute_forward_mul_mat
 // (ggml/src/ggml-cpu/ggml-cpu.c:1254-1452 -> ggml_vec_dot_q*_q8_* , ggml-cpu/quants.c:225-904); the closest analogue
@@ -16,7 +16,7 @@
 //     on-chip (ld*_a2 funnel shifts in qmm_formats.cuh).
 //   * Per segment a lane handles 2 of the 64 "units" of 32 weights: integer dp4a against the CPU-identical
 //     Q8_K/Q8_0 activations, one fp32 FMA per unit, warp-shuffle reduction at the end of the row.
-//   * Rows are dealt round-robin over CTAs (row r -> CTA r % grid), grid = 4 CTAs x 148 SMs, so every SM streams
+//   * Rows are dealt round-robin over CTAs (row r -> CTA r % grid), grid = 4 CTAs x 132 SMs, so every SM streams
 //     the same number of bytes +-1 row.
 #include "qmm_formats.cuh"
 #include "qmm_kernels.cuh"
@@ -156,7 +156,7 @@ static cudaError_t launch_one(const GemvArgs & a, cudaStream_t st) {
     if (!attr_done[dev & 63]) {
         cudaError_t e = cudaFuncSetAttribute(gemv_q_kernel<T, NCOLS>, cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM);
         if (e != cudaSuccess) return e;
-        int n = 148;
+        int n = 132;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
         sm_count[dev & 63] = n;
         attr_done[dev & 63] = true;

@@ -184,7 +184,7 @@ static cudaError_t launch2_one(const GemvArgs & a, cudaStream_t st) {
     cudaGetDevice(&dev);
     dev &= 63;
     if (sm_count[dev] == 0) {
-        int n = 148;
+        int n = 132;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
         sm_count[dev] = n;
     }

@@ -127,7 +127,7 @@ __global__ void __launch_bounds__(G2<T>::WARPS * 32) gemv3_kernel(const FusedGem
 
     // ---- keep HBM busy across the launch boundary: ask the L2 to start pulling in the NEXT launch's weights now.  A decode
     //      mat-vec is a latency chain (launch -> prologue -> first bytes -> compute -> tail) during which HBM mostly idles;
-    //      the next launch then finds its weights in the 126 MB L2.  Fire-and-forget bulk prefetches, one slice per CTA.
+    //      the next launch then finds its weights in the 50 MB L2.  Fire-and-forget bulk prefetches, one slice per CTA.
     if (warp == C::WARPS - 1) {
 #pragma unroll
         for (int m = 0; m < 3; m++) {
@@ -345,7 +345,7 @@ static cudaError_t launch3(const FusedGemvArgs & a, cudaStream_t st) {
     cudaGetDevice(&dev);
     dev &= 63;
     if (!attr[dev]) {
-        int n = 148;
+        int n = 132;
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
         sm_count[dev] = n;
         cudaError_t e = cudaFuncSetAttribute(gemv3_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024 - 512);   // the kernel also has a little static shared memory

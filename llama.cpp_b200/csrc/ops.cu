@@ -122,7 +122,7 @@ cudaError_t binary(int op, const TensorView & a, const TensorView & b, const Ten
     if (op < 2 && n % 4 == 0 && n >= 4096 && flat_f32(a) && flat_f32(b) && flat_f32(y) && a.ne[0] == b.ne[0] && a.ne[1] == b.ne[1] && a.ne[2] == b.ne[2] && a.ne[3] == b.ne[3] &&
         a.ne[0] == y.ne[0] && a.ne[1] == y.ne[1] && a.ne[2] == y.ne[2] && a.ne[3] == y.ne[3]) {
         const int64_t n4 = n / 4;
-        const unsigned grid = (unsigned)(cdiv(n4, 256) < 148 * 16 ? cdiv(n4, 256) : 148 * 16);
+        const unsigned grid = (unsigned)(cdiv(n4, 256) < 132 * 16 ? cdiv(n4, 256) : 132 * 16);
         binary_flat4_kernel<<<grid, 256, 0, st>>>(op, (const float4 *)a.data, (const float4 *)b.data, (float4 *)y.data, n4);
         return cudaGetLastError();
     }
@@ -351,7 +351,7 @@ cudaError_t swiglu(const TensorView & a, const TensorView * b, const TensorView 
     if (b != nullptr && !swapped && n % 4 == 0 && n >= 4096 && flat_f32(a) && flat_f32(*b) && flat_f32(y) && a.ne[0] == y.ne[0] && b->ne[0] == y.ne[0] &&
         a.ne[1] * a.ne[2] * a.ne[3] == y.ne[1] * y.ne[2] * y.ne[3] && b->ne[1] * b->ne[2] * b->ne[3] == y.ne[1] * y.ne[2] * y.ne[3]) {
         const int64_t n4 = n / 4;
-        const unsigned grid = (unsigned)(cdiv(n4, 256) < 148 * 16 ? cdiv(n4, 256) : 148 * 16);
+        const unsigned grid = (unsigned)(cdiv(n4, 256) < 132 * 16 ? cdiv(n4, 256) : 132 * 16);
         swiglu_flat4_kernel<<<grid, 256, 0, st>>>((const float4 *)a.data, (const float4 *)b->data, (float4 *)y.data, n4);
         return cudaGetLastError();
     }

@@ -1,4 +1,4 @@
-// qmm_formats.cuh -- GGUF block formats as seen by the B200 kernels.
+// qmm_formats.cuh -- GGUF block formats as seen by the kernels.
 //
 // Everything here is index arithmetic on the reference's on-disk block layouts
 // (ggml/src/ggml-common.h:194-376) plus the per-"unit" integer dot products the decode GEMV is built from.

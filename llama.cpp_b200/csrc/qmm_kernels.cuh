@@ -72,12 +72,12 @@ struct FusedGemvArgs {
     int             mode;             // 0 store, 1 + residual, 2 SwiGLU pair (dst[0] = silu(W0 x) * (W1 x))
     int             pdl;              // launch with programmatic stream serialisation
     unsigned *      counter;          // zeroed ticket counter for dynamic row-group distribution (nullptr = static split)
-    const uint8_t * next_w[3];        // weights of the NEXT fused launch: prefetched into the 126 MB L2 while this launch runs
+    const uint8_t * next_w[3];        // weights of the NEXT fused launch: prefetched into the 50 MB L2 while this launch runs
     int64_t         next_bytes[3];
 };
 cudaError_t launch_fused_gemv(int type, const FusedGemvArgs & a, cudaStream_t st);
 
-// Prefill GEMM (tcgen05): dst[M,N] = W[M,K] . X[K,N] with X pre-quantised to ActQ8-derived fp16 integer operands.
+// Prefill GEMM (wgmma): dst[M,N] = W[M,K] . X[K,N] with X pre-quantised to ActQ8-derived fp16 integer operands.
 struct GemmArgs {
     const uint8_t * w; int64_t row_stride; int M, K, N;
     const float * x; int64_t ldx;
@@ -87,7 +87,7 @@ struct GemmArgs {
 };
 size_t      gemm_workspace_bytes(int type, int64_t M, int64_t N, int64_t K);
 cudaError_t launch_gemm(int type, const GemmArgs & a, cudaStream_t st);
-// Q4_0 / Q8_0 (gemm_legacy_tcgen05.cu); launch_gemm and gemm_workspace_bytes dispatch to these
+// Q4_0 / Q8_0 (gemm_legacy_wgmma.cu); launch_gemm and gemm_workspace_bytes dispatch to these
 size_t      gemm_legacy_workspace_bytes(int type, int64_t M, int64_t N, int64_t K);
 cudaError_t launch_gemm_legacy(int type, const GemmArgs & a, cudaStream_t st);
 // grouped GEMM for MUL_MAT_ID with many tokens: w [K, M, n_expert], x columns [K] at x + (t * nb1 + (nb1 == 1 ? 0 : s)) * ldx, ids[t * ids_stride + s],
@@ -101,7 +101,6 @@ struct GemmGroupedArgs {
 };
 size_t      gemm_grouped_workspace_bytes(int type, int64_t M, int64_t jobs, int64_t n_expert, int64_t K);
 cudaError_t launch_gemm_grouped(int type, const GemmGroupedArgs & a, cudaStream_t st);
-void        set_gemm_variant(int v);   // 2 = warp-specialised pipelined kernel (default), 1 = first generation
 
 // ---- one-shot NVLink all-reduce (allreduce.cu), used by the backend's ggml_backend_comm_* hooks
 constexpr int ONESHOT_MAX_DEV = 8;

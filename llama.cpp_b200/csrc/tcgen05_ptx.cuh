@@ -1,6 +1,7 @@
-// tcgen05_ptx.cuh -- the PTX wrappers shared by the tcgen05 GEMM kernels (gemm_tcgen05.cu: K-quants, exact-integer operands;
-// gemm_legacy_tcgen05.cu: Q4_0 / Q8_0, hi/lo fp16 operands): mbarriers, 1-D bulk copies, TMEM allocation / loads, tcgen05.mma / commit /
-// fences, and the shared-memory and instruction descriptors of the canonical K-major SWIZZLE_128B layout.
+// tcgen05_ptx.cuh (a historical name) -- the PTX wrappers shared by the prefill GEMM kernels (gemm_tcgen05.cu: K-quants, exact-integer operands;
+// gemm_legacy_wgmma.cu: Q4_0 / Q8_0, hi/lo fp16 operands): mbarriers, 1-D bulk copies (TMA), the sm_90a warpgroup MMA
+// (wgmma.mma_async m64n128k16, fp16 in, fp32 accumulators in registers) and its fences, and the shared-memory descriptor of the
+// canonical K-major SWIZZLE_128B layout.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -27,52 +28,53 @@ __device__ __forceinline__ void g_bulk_g2s(void * dst, const void * src, uint32_
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
                  ::"r"(s32(dst)), "l"(src), "r"(bytes), "r"(s32(bar)) : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t * smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;\n" ::"r"(s32(smem_dst)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;\n" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;\n" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;\n" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;\n" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory"); }
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n"
-                 ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t * bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n" ::"r"(s32(bar)) : "memory");
-}
-// 32 lanes x 32 columns of 32-bit: thread i of the warp gets lane (base + i), columns c..c+31
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float * v) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, "
-        "%22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];\n"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]),
-          "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]),
-          "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
+// barrier among the 128 threads of one warpgroup (ids 1.. are free: __syncthreads uses 0)
+__device__ __forceinline__ void wg_bar_sync(int wg) { asm volatile("bar.sync %0, 128;\n" ::"r"(1 + wg) : "memory"); }
+
+// ------------------------------------------------------------------------------------------------ warpgroup MMA
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;\n" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;\n" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;\n" ::"n"(N) : "memory"); }
+// Pins the accumulator registers at this point of the program: the compiler may not move their reads above a wgmma_wait or
+// their writes below the wgmma that follows.
+__device__ __forceinline__ void acc_fence(float (&d)[64]) {
 #pragma unroll
-    for (int i = 0; i < 32; i++) v[i] = __uint_as_float(r[i]);
+    for (int i = 0; i < 64; i++) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, mma_sm100_desc.hpp): start address
-// >> 4 in bits [0,14), LBO (unused for swizzled K-major) = 1 in [16,30), SBO = 1024 B (8 rows x 128 B) >> 4 in [32,46),
-// version = 1 in [46,48), layout type SWIZZLE_128B = 2 in [61,64).
+// D[64 x 128] (+)= A[64 x 16] . B[128 x 16]^T, both K-major in shared memory, fp16 in, fp32 accumulate.  Thread t of the warpgroup
+// holds rows 16 (t / 32) + (t % 32) / 4 (+ 8) and columns 8 i + 2 (t % 4) (+ 1): d[4 i + 2 hi + c] = D[row + 8 hi][8 i + 2 (t % 4) + c].
+__device__ __forceinline__ void wgmma_m64n128k16_f16(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, "
+        "%29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, "
+        "%56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]),
+          "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]),
+          "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]),
+          "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]),
+          "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]),
+          "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate)
+        : "memory");
+}
+
+// K-major SWIZZLE_128B shared-memory matrix descriptor of sm_90 (cute::GMMA::DescriptorSM90): start address >> 4 in bits [0,14),
+// LBO (unused for swizzled K-major) = 1 in [16,30), SBO = 1024 B (8 rows x 128 B) >> 4 in [32,46), base offset 0 (atoms are
+// 1024-byte aligned), layout type SWIZZLE_128B = 1 in [62,64).  A k16 slice inside the 128-byte row is selected by adding its byte
+// offset (32 per slice) to the start address.
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr) {
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);
     d |= (uint64_t)1 << 16;
     d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = F32 (1 << 4), A = B = F16 (0), K-major both, N >> 3 at [17,23), M >> 4 at [24,29)
-__host__ __device__ constexpr uint32_t make_idesc_f16(int m, int n) { return (1u << 4) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(m >> 4) << 24); }
-
 
 }  // namespace qmm

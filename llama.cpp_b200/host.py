@@ -1,7 +1,7 @@
 """ctypes binding of include/b200_qmm.h for the Python harness.
 
 torch is used for device memory and streams only; every computation is a call into libb200qmm.so.  If the library
-is missing, or there is no sm_100 device, the calls raise -- there is no eager / CPU fallback."""
+is missing, or there is no sm_90 device, the calls raise -- there is no eager / CPU fallback."""
 from __future__ import annotations
 
 import ctypes as C
@@ -45,7 +45,6 @@ def lib() -> C.CDLL:
         L.b200_mul_mat.argtypes = [ci, vp, i64, i64, i64, vp, i64, i64, vp, i64, vp, sz, vp]
         L.b200_set_mul_mat_path.argtypes = [ci]
         L.b200_set_gemv_variant.argtypes = [ci]
-        L.b200_set_gemm_variant.argtypes = [ci]
         L.b200_matvec_program.argtypes = [ci] + [C.c_void_p] * 12 + [C.c_void_p]
         L.b200_matvec_program.restype = ci
         L.b200_gemv_q8.argtypes = [ci, vp, i64, i64, i64, vp, i64, vp, i64, vp]

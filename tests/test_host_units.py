@@ -69,5 +69,5 @@ def test_dequant_elem_bit_exact(hu, oracle, t):
 
 def test_gemm_prepass_chunk_layout(hu):
     """The warp-per-block activation pre-pass stores one 16-byte chunk per lane; its element order and address must equal the
-    per-element swizzled K-major addressing (gemm_layout.cuh) that the weight de-quantiser and the tcgen05 descriptors assume."""
+    per-element swizzled K-major addressing (gemm_layout.cuh) that the weight de-quantiser and the wgmma descriptors assume."""
     assert hu.hu_prepass_layout_mismatches(128) == 0

@@ -1,4 +1,4 @@
-"""Diagnostic (GPU box): per-node comparison CPU vs B200 through llama's cb_eval hook, and logits error matrix."""
+"""Diagnostic (GPU box): per-node comparison CPU vs GPU through llama's cb_eval hook, and logits error matrix."""
 import ctypes as C, os, subprocess, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -12,7 +12,7 @@ def run(tag, ngl, fa, dump, extra_env=None):
     env = dict(os.environ); env.update(extra_env or {})
     code = f"""
 import ctypes as C, numpy as np, os
-L = C.CDLL({os.path.join(ROOT, 'tools', 'libllama_host.so')!r})
+L = C.CDLL({os.path.join(ROOT, 'oracle', '_ref', 'host', 'libllama_host.so')!r})
 L.lh_open.restype = C.c_void_p
 L.lh_open.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_char_p]
 L.lh_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]

@@ -1,4 +1,4 @@
-"""GPU tuning aid: achieved TFLOP/s of the prefill GEMM (activation pre-pass + tcgen05 kernel) per shape."""
+"""GPU tuning aid: achieved TFLOP/s of the prefill GEMM (activation pre-pass + wgmma kernel) per shape."""
 import json, os, sys
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

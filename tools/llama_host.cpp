@@ -1,9 +1,9 @@
-// llama_host.cpp -- a minimal driver over the REFERENCE's unmodified libllama (host/_ref/libllama.so) that exposes
+// llama_host.cpp -- a minimal driver over the REFERENCE's unmodified libllama (built by oracle/host.mk) that exposes
 // what llama-bench measures (tools/llama-bench/llama-bench.cpp:2114-2162: test_prompt = llama_decode per n_batch chunk
 // + one llama_synchronize; test_gen = llama_decode of 1 token + llama_synchronize per token) as a small C API that
-// bench.py and the parity tests call through ctypes, plus a CLI.  (The unmodified llama-bench itself is built by host/Makefile too
+// bench.py and the parity tests call through ctypes, plus a CLI.  (The unmodified llama-bench itself is built by oracle/host.mk too
 // and reported beside these numbers; this driver exists for what llama-bench has no hooks for: logits out, cb_eval dumps, device
-// replay.)  libllama, ggml and the backend registry it drives are the reference's own code, compiled unmodified by host/Makefile.
+// replay.)  libllama, ggml and the backend registry it drives are the reference's own code, compiled unmodified by oracle/host.mk.
 //
 // The backend under test is selected exactly as a user would: GGML_BACKEND_PATH=/path/libggml-b200.so makes
 // ggml_backend_load_all() dlopen the plugin (ggml-backend-reg.cpp:566-593); n_gpu_layers > 0 offloads to it.

@@ -2,7 +2,7 @@
 """Random-init Llama/Mixtral GGUF files for the parity harness and the benchmark (SURVEY.md section 8d recipe).
 
   --quant exact   weights ~ N(0, 0.02) quantised per tensor by the REFERENCE quantiser (ggml_quantize_chunk of the reference
-                  host's own libggml-base, host/_ref -- what llama-quantize calls per tensor)
+                  host's own libggml-base.so, found on LD_LIBRARY_PATH -- what llama-quantize calls per tensor)
                   with llama-quant.cpp's Q4_K_M / Q5_K_M / Q4_0 type mix -- for logits parity on small models
   --quant synth   random valid blocks written directly (no f32 weights, no quantiser) -- for 8B/70B-sized bench files
 
@@ -23,7 +23,6 @@ from gguf import GGMLQuantizationType as QT  # noqa: E402
 Q4_0, Q8_0, Q4_K, Q5_K, Q6_K = 2, 8, 12, 13, 14
 BLOCK_ELEMS = {Q4_0: 32, Q8_0: 32, Q4_K: 256, Q5_K: 256, Q6_K: 256}
 BLOCK_BYTES = {Q4_0: 18, Q8_0: 34, Q4_K: 144, Q5_K: 176, Q6_K: 210}
-HOST_REF = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "host", "_ref")
 
 
 def random_blocks(t, rows, k, rng, scale=0.02):
@@ -51,12 +50,12 @@ def random_blocks(t, rows, k, rng, scale=0.02):
 
 
 class HostQuantiser:
-    """ggml_quantize_chunk (ggml/src/ggml.c) from the reference host's libggml-base.so."""
+    """ggml_quantize_chunk (ggml/src/ggml.c) from the reference host's libggml-base.so (the one the dynamic loader finds)."""
 
     def __init__(self):
         import ctypes as C
         self.C = C
-        self.lib = C.CDLL(os.path.join(HOST_REF, "libggml-base.so"))
+        self.lib = C.CDLL("libggml-base.so")
         self.lib.ggml_quantize_chunk.restype = C.c_size_t
         self.lib.ggml_quantize_chunk.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int64, C.c_void_p]
 

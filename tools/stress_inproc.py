@@ -20,7 +20,7 @@ os.environ["GGML_BACKEND_PATH"] = os.path.join(ROOT, "llama.cpp_b200", "libggml-
 gguf = f"/tmp/stress_{preset}_{ftype}.gguf"
 if not os.path.exists(gguf):
     subprocess.check_call([sys.executable, os.path.join(ROOT, "tools", "make_gguf.py"), gguf, "--preset", preset, "--ftype", ftype])
-L = C.CDLL(os.path.join(ROOT, "tools", "libllama_host.so"))
+L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "host", "libllama_host.so"))
 L.lh_open.restype = C.c_void_p
 L.lh_open.argtypes = [C.c_char_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_char_p]
 L.lh_decode.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]

@@ -4,7 +4,7 @@ import ctypes as C, os, subprocess, sys
 import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PLUGIN = os.path.join(ROOT, "llama.cpp_b200", "libggml-b200.so")
-HOSTLIB = os.path.join(ROOT, "tools", "libllama_host.so")
+HOSTLIB = os.path.join(ROOT, "oracle", "_ref", "host", "libllama_host.so")
 gguf = "/tmp/tp_small.gguf"
 subprocess.check_call([sys.executable, os.path.join(ROOT, "tools", "make_gguf.py"), gguf, "--preset", "small", "--ftype", "q4_k_m"])
 toks = np.random.default_rng(3).integers(0, 512, size=20)

@@ -1,8 +1,8 @@
-// Micro-benchmark (sm_100a): HBM -> shared memory throughput of cp.async.bulk as a function of who issues the copies.
+// Micro-benchmark (sm_90a; nvcc -O3 -gencode arch=compute_90a,code=sm_90a): HBM -> shared memory throughput of cp.async.bulk as a function of who issues the copies.
 // One CTA per SM; W warps x L lanes are "issuers"; every issuer streams its own disjoint part of a large buffer through its own
 // ring of D slots of S bytes (one mbarrier per slot; the data is not consumed -- a slot is re-armed as soon as its copy has landed).
 // Prints achieved TB/s over the whole chip.  Question it answers: does a decode kernel need MANY issuing lanes / warps, or deep rings,
-// or large copies, to keep 148 SMs' share of HBM busy?
+// or large copies, to keep every SM's share of HBM busy?
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-// hop_latency.cu -- how long does a tagged-slot vector take from one CTA's stores to every other CTA having read it, while every
+// hop_latency.cu (sm_90a; nvcc -O3 -gencode arch=compute_90a,code=sm_90a) -- how long does a tagged-slot vector take from one CTA's stores to every other CTA having read it, while every
 // SM streams weights with cp.async.bulk?  (The persistent decode kernel pays this once per phase: 160 times per token.)
 //
 //   hop_latency <cap> <poll_mode> <rounds> [n_slots]
@@ -123,7 +123,7 @@ __global__ void set_stop(int * stop) { *stop = 1; }
 int main(int argc, char ** argv) {
     const int cap = argc > 1 ? atoi(argv[1]) : 0, mode = argc > 2 ? atoi(argv[2]) : 0, rounds = argc > 3 ? atoi(argv[3]) : 600, n_slots = argc > 4 ? atoi(argv[4]) : 4096;
     if (cap > MAXCAP || n_slots > 2 * 32 * CTHREADS) { fprintf(stderr, "cap <= %d, n_slots <= %d\n", MAXCAP, 2 * 32 * CTHREADS); return 2; }
-    int grid = 148;
+    int grid = 132;
     cudaDeviceGetAttribute(&grid, cudaDevAttrMultiProcessorCount, 0);
     const size_t wbytes = (size_t)4 << 30;
     uint8_t * w; uint64_t * slots; unsigned long long * t_w, * t_r, * copied; int * stop;

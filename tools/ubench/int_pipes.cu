@@ -1,9 +1,9 @@
-// Micro-benchmark (sm_100a): issue rate of the integer dot-product paths a quantised GEMV can use.
+// Micro-benchmark (sm_90a; nvcc -O3 -gencode arch=compute_90a,code=sm_90a): issue rate of the integer dot-product paths a quantised GEMV can use.
 //   dp4a            IDP.4A on the CUDA cores (what round 1's decode kernels were built on)
 //   imad            IMAD (full-rate integer pipe), for scale
 //   mma.s8 k32      mma.sync.m16n8k32 s8 x s8 -> s32 (legacy tensor-core path)
 //   mma.f16 k16     mma.sync.m16n8k16 f16 x f16 -> f32
-//   fma.f32x2 / ffma  packed and scalar fp32 FMA (the prefill GEMM's epilogue runs on the packed form)
+//   ffma            scalar fp32 FMA (the prefill GEMMs' per-block rescale)
 // Every warp runs `iters` x 16 independent chains; prints warp-instructions per cycle per SM for 1, 2, 4, 8 warps per SMSP.
 #include <cstdio>
 #include <cstdint>
@@ -28,11 +28,6 @@ __global__ void bench(int iters, unsigned long long * cycles, int * sink) {
                 asm volatile("mma.sync.aligned.m16n8k32.row.col.s32.s8.s8.s32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};\n"
                              : "+r"(c0), "+r"(c1), "+r"(c2), "+r"(c3) : "r"(a), "r"(a + 1), "r"(a + 2), "r"(a + 3), "r"(b), "r"(b + 1));
                 acc[i] = c0 + c1 + c2 + c3;
-            }
-            if (MODE == 4) {
-                unsigned long long v = ((unsigned long long)__float_as_uint(facc[i]) << 32) | __float_as_uint(facc[i] + 1.0f), w = 0x3f8000003f800000ull, r;
-                asm volatile("fma.rn.f32x2 %0, %1, %2, %1;\n" : "=l"(r) : "l"(v), "l"(w));
-                facc[i] = __uint_as_float((unsigned)(r >> 32));
             }
             if (MODE == 5) facc[i] = fmaf(facc[i], 1.0001f, 0.5f);
             if (MODE == 3) {
@@ -84,7 +79,6 @@ int main() {
     run<1>("imad", sms);
     run<2>("mma.s8.k32", sms);
     run<3>("mma.f16.k16", sms);
-    run<4>("fma.f32x2", sms);
     run<5>("ffma", sms);
     return 0;
 }
