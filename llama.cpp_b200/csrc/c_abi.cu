@@ -1,4 +1,4 @@
-// c_abi.cu -- the extern "C" surface declared in include/b200_qmm.h.  Thin: argument checks, workspace carving,
+// c_abi.cu -- the extern "C" surface declared in include/b200_qmm.h and include/b200_attn.h.  Thin: argument checks, workspace carving,
 // regime selection (decode GEMV vs prefill GEMM), error text.  No compute happens on the host and there is no CPU
 // fallback: if CUDA is unusable every compute entry point fails loudly.
 #include <atomic>
@@ -7,10 +7,13 @@
 #include <mutex>
 
 #include "../../include/b200_qmm.h"
+#include "../../include/b200_attn.h"
 #include "qmm_formats.cuh"
 #include <vector>
 #include <string.h>
 #include "qmm_kernels.cuh"
+#include "qmm_ops.cuh"
+#include "qmm_attn.cuh"
 #include "decode_flow.cuh"
 
 namespace qmm {
@@ -147,29 +150,49 @@ int b200_fused_matvec(int type, int nmat, const void * const * w, const int64_t 
     return from_cuda(launch_fused_gemv(type, a, (cudaStream_t)stream), "b200_fused_matvec");
 }
 
-int b200_matvec_program(int n, const int * type, const int * nmat, const void * const * w, const int64_t * row_stride, const int64_t * M,
-                        const int64_t * K, const float * const * x, const float * const * norm_w, const float * eps, const int * mode,
-                        const float * const * residual, float * const * dst, void * stream) {
-    if (n <= 0 || n > 1024) return fail(B200_E_INVALID, "b200_matvec_program: bad phase count");
-    // per-device program buffer, tagged-slot pool and zeroed sync words; the previous program may still be running on another
-    // stream: callers serialise on the device
+// Per-device program buffer, tagged-slot pool and zeroed sync words of the programs launched through this C ABI
+// (b200_matvec_program, b200_attn_program).  The previous program may still be running on another stream: callers serialise
+// on the device.
+struct FlowBuffers { FlowPhase * ph; unsigned * sync; uint64_t * ll; int dev; };
+constexpr int FLOW_ABI_PHASES = 1024;
+constexpr size_t FLOW_ABI_LL_ELEMS = 512 * 1024;
+
+static cudaError_t flow_buffers(FlowBuffers & fbuf) {
     static FlowPhase * d_ph[64] = {};
     static unsigned * d_sync[64] = {};
     static uint64_t * d_ll[64] = {};
-    constexpr size_t LL_ELEMS = 512 * 1024;
     int dev = 0;
     cudaGetDevice(&dev);
     dev &= 63;
     if (!d_ph[dev]) {
-        if (cudaMalloc(&d_ph[dev], 1024 * sizeof(FlowPhase)) != cudaSuccess || cudaMalloc(&d_sync[dev], flow_sync_bytes()) != cudaSuccess ||
-            cudaMalloc(&d_ll[dev], LL_ELEMS * sizeof(uint64_t)) != cudaSuccess) return from_cuda(cudaGetLastError(), "b200_matvec_program(alloc)");
+        if (cudaMalloc(&d_ph[dev], FLOW_ABI_PHASES * sizeof(FlowPhase)) != cudaSuccess || cudaMalloc(&d_sync[dev], flow_sync_bytes()) != cudaSuccess ||
+            cudaMalloc(&d_ll[dev], FLOW_ABI_LL_ELEMS * sizeof(uint64_t)) != cudaSuccess) return cudaGetLastError();
         cudaMemset(d_sync[dev], 0, flow_sync_bytes());
-        cudaMemset(d_ll[dev], 0, LL_ELEMS * sizeof(uint64_t));
+        cudaMemset(d_ll[dev], 0, FLOW_ABI_LL_ELEMS * sizeof(uint64_t));
         cudaDeviceSynchronize();                               // the caller's stream may be non-blocking: order the zeroing before its first launch
     }
+    fbuf.ph = d_ph[dev]; fbuf.sync = d_sync[dev]; fbuf.ll = d_ll[dev]; fbuf.dev = dev;
+    return cudaSuccess;
+}
+
+static cudaError_t flow_launch(const FlowBuffers & fbuf, const FlowBuilder & fb, cudaStream_t st) {
+    const int n = (int)fb.size();
+    cudaError_t e = cudaMemcpyAsync(fbuf.ph, fb.phases().data(), (size_t)n * sizeof(FlowPhase), cudaMemcpyHostToDevice, st);
+    if (e != cudaSuccess) return e;
+    FlowProgram prog{fbuf.ph, n, fbuf.sync, 0, nullptr};
+    return launch_decode_flow(prog, st);
+}
+
+int b200_matvec_program(int n, const int * type, const int * nmat, const void * const * w, const int64_t * row_stride, const int64_t * M,
+                        const int64_t * K, const float * const * x, const float * const * norm_w, const float * eps, const int * mode,
+                        const float * const * residual, float * const * dst, void * stream) {
+    if (n <= 0 || n > FLOW_ABI_PHASES) return fail(B200_E_INVALID, "b200_matvec_program: bad phase count");
+    FlowBuffers fbuf;
+    cudaError_t e = flow_buffers(fbuf);
+    if (e != cudaSuccess) return from_cuda(e, "b200_matvec_program(alloc)");
     // the same builder the ggml backend uses: a phase whose input is an earlier phase's output reads it through tagged slots
     FlowBuilder fb;
-    fb.reset(d_ll[dev], LL_ELEMS, flow_grid(dev));
+    fb.reset(fbuf.ll, FLOW_ABI_LL_ELEMS, flow_grid(fbuf.dev));
     for (int i = 0; i < n; i++) {
         FlowBuilder::MatvecDesc d;
         d.nmat = nmat[i]; d.K = (int)K[i]; d.mode = mode[i]; d.x = x[i]; d.norm_w = norm_w[i]; d.eps = eps[i]; d.residual = residual[i];
@@ -178,11 +201,95 @@ int b200_matvec_program(int n, const int * type, const int * nmat, const void * 
         }
         if (!fb.add_matvec(d)) return fail(B200_E_INVALID, "b200_matvec_program: phase not supported");
     }
+    return from_cuda(flow_launch(fbuf, fb, (cudaStream_t)stream), "b200_matvec_program");
+}
+
+int b200_attn_program(const b200_attn_args * a, int * nsplit, void * stream) {
+    if (a == nullptr) return fail(B200_E_INVALID, "b200_attn_program: no arguments");
+    if (a->head_dim != 128) return fail(B200_E_UNSUPPORTED, "b200_attn_program: head_dim must be 128");
+    if (a->n_head <= 0 || a->n_head_kv <= 0 || a->n_head % a->n_head_kv) return fail(B200_E_INVALID, "b200_attn_program: n_head must be a multiple of n_head_kv");
+    if (a->n_kv <= 0 || a->n_dims <= 0 || a->n_dims > a->head_dim || a->n_dims % 2 || (a->rope_mode != 0 && a->rope_mode != 2))
+        return fail(B200_E_INVALID, "b200_attn_program: bad n_kv / n_dims / rope mode");
+    if (!a->q || !a->k || !a->v || !a->dst || !a->pos || !a->kpos || !a->vpos || !a->k_cache || !a->v_cache || !a->kview || !a->vview)
+        return fail(B200_E_INVALID, "b200_attn_program: missing pointer");
+    const bool fused = a->w_qkv[0] != nullptr;
+    if (fused && (!a->w_qkv[1] || !a->w_qkv[2] || !a->x || a->n_embd <= 0 || a->n_embd > INT32_MAX))
+        return fail(B200_E_INVALID, "b200_attn_program: incomplete q|k|v mat-vec");
+    FlowBuffers fbuf;
+    cudaError_t e = flow_buffers(fbuf);
+    if (e != cudaSuccess) return from_cuda(e, "b200_attn_program(alloc)");
+    FlowBuilder fb;
+    fb.reset(fbuf.ll, FLOW_ABI_LL_ELEMS, flow_grid(fbuf.dev));
+    if (fused) {
+        FlowBuilder::MatvecDesc d;
+        d.nmat = 3; d.K = (int)a->n_embd; d.mode = 0; d.x = a->x; d.norm_w = a->norm_w; d.eps = a->eps;
+        float * outs[3] = {a->q, a->k, a->v};
+        const int64_t rows[3] = {(int64_t)a->head_dim * a->n_head, (int64_t)a->head_dim * a->n_head_kv, (int64_t)a->head_dim * a->n_head_kv};
+        for (int j = 0; j < 3; j++) {
+            d.w[j] = (const uint8_t *)a->w_qkv[j]; d.row_stride[j] = a->row_stride_qkv[j]; d.M[j] = (int)rows[j]; d.type[j] = a->type_qkv[j]; d.dst[j] = outs[j];
+        }
+        if (!fb.add_matvec(d)) return fail(B200_E_UNSUPPORTED, "b200_attn_program: q|k|v mat-vec not representable");
+    }
+    // FlowAttn as the backend fills it for a ROPE pair + SET_ROWS pair + FLASH_ATTN_EXT (backend/ggml_b200.cpp, fuse_rope_pair)
+    ops::RopeKVArgs r{};
+    r.n_dims = a->n_dims; r.n_ctx_orig = a->n_ctx_orig; r.freq_base = a->freq_base; r.beta_fast = a->beta_fast; r.beta_slow = a->beta_slow;
+    FlowAttn m;
+    memset(&m, 0, sizeof(m));
+    m.k_cache = a->k_cache; m.k_row_bytes = a->k_row_bytes; m.v_cache = a->v_cache; m.v_row_bytes = a->v_row_bytes;
+    m.k_idx = a->kpos; m.v_idx = a->vpos; m.pos = a->pos; m.freq_factors = a->freq_factors;
+    m.kview = a->kview; m.k_nb1 = a->k_nb1; m.k_nb2 = a->k_nb2;
+    m.vview = a->vview; m.v_nb1 = a->v_nb1; m.v_nb2 = a->v_nb2;
+    m.mask = a->mask;
+    m.n_head = a->n_head; m.n_head_kv = a->n_head_kv; m.head_dim = a->head_dim; m.n_dims = a->n_dims; m.rope_mode = a->rope_mode; m.n_kv = a->n_kv;
+    m.freq_scale = a->freq_scale; m.ext_factor = a->ext_factor; m.attn_factor = a->attn_factor;
+    ops::rope_derived(r, m.theta_scale, m.corr0, m.corr1);
+    m.softcap = a->softcap; m.scale = a->softcap != 0.0f ? a->scale / a->softcap : a->scale;
+    if (!fb.add_attn(m, a->q, a->k, a->v, a->dst)) return fail(B200_E_UNSUPPORTED, "b200_attn_program: attention phase not representable");
+    if (nsplit) *nsplit = fb.phases().back().at.nsplit;
+    return from_cuda(flow_launch(fbuf, fb, (cudaStream_t)stream), "b200_attn_program");
+}
+
+static ops::TensorView tview(const void * p, const int64_t * ne, const int64_t * nb, int type) {
+    ops::TensorView t;
+    t.data = const_cast<void *>(p);
+    for (int i = 0; i < 4; i++) { t.ne[i] = ne[i]; t.nb[i] = nb ? nb[i] : 0; }
+    t.type = type;
+    return t;
+}
+
+size_t b200_flash_attn_workspace_bytes(const int64_t * q_ne, const int64_t * k_ne, const int64_t * mask_ne) {
+    if (!q_ne || !k_ne) return 0;
+    const ops::TensorView q = tview(nullptr, q_ne, nullptr, 0), k = tview(nullptr, k_ne, nullptr, 1);
+    if (!mask_ne) return ops::flash_attn_workspace_bytes(q, k, nullptr);
+    const ops::TensorView m = tview(nullptr, mask_ne, nullptr, 1);
+    return ops::flash_attn_workspace_bytes(q, k, &m);
+}
+
+int b200_flash_attn(const float * q, const int64_t * q_ne, const int64_t * q_nb, const void * k, const int64_t * k_ne, const int64_t * k_nb,
+                    const void * v, const int64_t * v_ne, const int64_t * v_nb, const void * mask, const int64_t * mask_ne, const int64_t * mask_nb,
+                    float * dst, const int64_t * dst_ne, const int64_t * dst_nb, float scale, float softcap, void * ws, size_t ws_bytes, int path, void * stream) {
+    if (!q_ne || !q_nb || !k_ne || !k_nb || !v_ne || !v_nb || !dst_ne || !dst_nb || (mask && (!mask_ne || !mask_nb)) || path < 0 || path > 2)
+        return fail(B200_E_INVALID, "b200_flash_attn: bad arguments");
+    for (int i = 0; i < 4; i++)
+        if (q_ne[i] <= 0 || k_ne[i] <= 0 || v_ne[i] <= 0 || (mask && mask_ne[i] <= 0)) return fail(B200_E_INVALID, "b200_flash_attn: empty dimension");
+    const int64_t DK = q_ne[0], N = q_ne[1], H = q_ne[2], B = q_ne[3], n_kv = k_ne[1], DV = v_ne[0];
+    if (k_ne[0] != DK || v_ne[1] != n_kv || H % k_ne[2] || H % v_ne[2] || B % k_ne[3] || B % v_ne[3])
+        return fail(B200_E_INVALID, "b200_flash_attn: q / k / v shapes do not broadcast");
+    if (dst_ne[0] != DV || dst_ne[1] != H || dst_ne[2] != N || dst_ne[3] != B) return fail(B200_E_INVALID, "b200_flash_attn: dst must be [DV, H, N, B]");
+    if (q_nb[0] != 4 || k_nb[0] != 2 || v_nb[0] != 2 || dst_nb[0] != 4 || (mask && mask_nb[0] != 2)) return fail(B200_E_INVALID, "b200_flash_attn: rows must be contiguous");
+    if (mask && (mask_ne[0] < n_kv || mask_ne[1] < N || H % mask_ne[2] || B % mask_ne[3])) return fail(B200_E_INVALID, "b200_flash_attn: mask shape");
+    if (path == 1 && (DK != DV || DK % 32 || DK > 256)) return fail(B200_E_UNSUPPORTED, "b200_flash_attn: the scalar kernel needs D = DV, a multiple of 32 up to 256");
+    if (path == 2 && (DK != DV || (DK != 64 && DK != 128) || N < ops::FA_MIN_ROWS_MMA))
+        return fail(B200_E_UNSUPPORTED, "b200_flash_attn: the tensor-core kernel needs D = DV in {64, 128} and >= 16 rows");
+    const ops::TensorView tq = tview(q, q_ne, q_nb, 0), tk = tview(k, k_ne, k_nb, 1), tv = tview(v, v_ne, v_nb, 1), td = tview(dst, dst_ne, dst_nb, 0);
+    const ops::TensorView tm = mask ? tview(mask, mask_ne, mask_nb, 1) : tq;
+    const ops::TensorView * pm = mask ? &tm : nullptr;
     cudaStream_t st = (cudaStream_t)stream;
-    cudaError_t e = cudaMemcpyAsync(d_ph[dev], fb.phases().data(), (size_t)n * sizeof(FlowPhase), cudaMemcpyHostToDevice, st);
-    if (e != cudaSuccess) return from_cuda(e, "b200_matvec_program(upload)");
-    FlowProgram prog{d_ph[dev], n, d_sync[dev], 0, nullptr};
-    return from_cuda(launch_decode_flow(prog, st), "b200_matvec_program");
+    cudaError_t e;
+    if (path == 0) e = ops::flash_attn(tq, tk, tv, pm, td, scale, softcap, st, ws, ws_bytes);
+    else if (path == 1) e = ops::flash_attn_scalar(tq, tk, tv, pm, td, scale, softcap, st);
+    else e = ops::flash_attn_prefill(tq, tk, tv, pm, td, scale, softcap, ws, ws_bytes, st);
+    return from_cuda(e, "b200_flash_attn");
 }
 
 size_t b200_flow_slot_bytes(void) { return flow_slot_bytes(); }

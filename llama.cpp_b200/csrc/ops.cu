@@ -8,6 +8,7 @@
 #include "qmm_formats.cuh"
 #include "qmm_kernels.cuh"
 #include "qmm_ops.cuh"
+#include "qmm_attn.cuh"
 
 namespace qmm {
 namespace ops {
@@ -467,11 +468,16 @@ static bool fa_mma_enabled() {
 
 cudaError_t flash_attn(const TensorView & q, const TensorView & k, const TensorView & v, const TensorView * mask, const TensorView & dst,
                        float scale, float softcap, cudaStream_t st, void * ws, size_t ws_bytes) {
-    const int D = (int)q.ne[0];
     if (q.ne[1] >= FA_MIN_ROWS_MMA && fa_mma_enabled()) {
         const cudaError_t pe = flash_attn_prefill(q, k, v, mask, dst, scale, softcap, ws, ws_bytes, st);
         if (pe != cudaErrorNotSupported) return pe;
     }
+    return flash_attn_scalar(q, k, v, mask, dst, scale, softcap, st);
+}
+
+cudaError_t flash_attn_scalar(const TensorView & q, const TensorView & k, const TensorView & v, const TensorView * mask, const TensorView & dst,
+                              float scale, float softcap, cudaStream_t st) {
+    const int D = (int)q.ne[0];
     if (D != (int)v.ne[0] || D % 32 || D > 256 || k.type != TY_F16 || v.type != TY_F16 || q.type != TY_F32) return cudaErrorNotSupported;
     if (q.ne[1] * q.ne[2] * q.ne[3] == 0) return cudaSuccess;
     if (softcap != 0.0f) scale /= softcap;

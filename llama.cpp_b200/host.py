@@ -55,6 +55,11 @@ def lib() -> C.CDLL:
         L.b200_mul_mat_host_scratch_bytes.restype = sz
         L.b200_mul_mat_host_scratch_bytes.argtypes = [ci, i64, i64, i64]
         L.b200_mul_mat_host.argtypes = [ci, vp, i64, i64, i64, vp, i64, vp, vp, sz, vp]
+        I4 = C.POINTER(i64)
+        L.b200_flash_attn_workspace_bytes.restype = sz
+        L.b200_flash_attn_workspace_bytes.argtypes = [I4, I4, I4]
+        L.b200_flash_attn.argtypes = [vp, I4, I4] * 5 + [C.c_float, C.c_float, vp, sz, ci, vp]
+        L.b200_attn_program.argtypes = [C.POINTER(AttnArgs), C.POINTER(ci), vp]
         _lib = L
     return _lib
 
@@ -179,6 +184,83 @@ def matvec_program(phases):
         PT(*[p["norm_w"].data_ptr() if p.get("norm_w") is not None else None for p in phases]), FA(*[p.get("eps", 1e-5) for p in phases]),
         IA(*[p.get("mode", 0) for p in phases]), PT(*[p["residual"].data_ptr() if p.get("residual") is not None else None for p in phases]),
         P3(*d3), _stream()), "b200_matvec_program")
+
+
+def _ggml_view(t: torch.Tensor | None):
+    """A torch tensor (any strides, <= 4 dims, outermost first) as ggml's (data, ne[4], nb[4] in bytes)."""
+    if t is None:
+        return None, None, None
+    assert t.dim() <= 4
+    shape = [1] * (4 - t.dim()) + list(t.shape)
+    stride = [0] * (4 - t.dim()) + list(t.stride())
+    ne = (C.c_int64 * 4)(*shape[::-1])
+    nb = (C.c_int64 * 4)(*[s * t.element_size() for s in stride[::-1]])
+    return t.data_ptr(), ne, nb
+
+
+def flash_attn_workspace_bytes(q: torch.Tensor, k: torch.Tensor, mask: torch.Tensor | None) -> int:
+    return int(lib().b200_flash_attn_workspace_bytes(_ggml_view(q)[1], _ggml_view(k)[1], _ggml_view(mask)[1]))
+
+
+def flash_attn(q, k, v, mask, dst, scale: float, softcap: float = 0.0, ws: torch.Tensor | None = None, path: int = 0) -> torch.Tensor:
+    """FLASH_ATTN_EXT (b200_flash_attn).  Tensors outermost dimension first, ggml's order reversed: q f32 [B, H, N, D], k / v f16
+    [Bk, Hkv, n_kv, D], mask f16 [m3, m2, >= N, >= n_kv] or None, dst f32 [B, N, H, DV]; any strides (views of a cache,
+    llama's permuted q).  path 0 auto, 1 scalar kernel, 2 tensor-core kernel; ws: scratch for the tile pre-pass or None."""
+    args = []
+    for t in (q, k, v, mask, dst):
+        args += list(_ggml_view(t))
+    _check(lib().b200_flash_attn(*args, scale, softcap, ws.data_ptr() if ws is not None else None, ws.numel() if ws is not None else 0, path,
+                                 _stream()), "b200_flash_attn")
+    return dst
+
+
+class AttnArgs(C.Structure):
+    """include/b200_qmm.h: b200_attn_args."""
+    _fields_ = [("type_qkv", C.c_int * 3), ("w_qkv", C.c_void_p * 3), ("row_stride_qkv", C.c_int64 * 3),
+                ("x", C.c_void_p), ("norm_w", C.c_void_p), ("n_embd", C.c_int64), ("eps", C.c_float),
+                ("q", C.c_void_p), ("k", C.c_void_p), ("v", C.c_void_p),
+                ("n_head", C.c_int), ("n_head_kv", C.c_int), ("head_dim", C.c_int), ("n_dims", C.c_int), ("rope_mode", C.c_int), ("n_ctx_orig", C.c_int),
+                ("freq_base", C.c_float), ("freq_scale", C.c_float), ("ext_factor", C.c_float), ("attn_factor", C.c_float),
+                ("beta_fast", C.c_float), ("beta_slow", C.c_float),
+                ("freq_factors", C.c_void_p), ("pos", C.c_void_p),
+                ("k_cache", C.c_void_p), ("k_row_bytes", C.c_int64), ("v_cache", C.c_void_p), ("v_row_bytes", C.c_int64),
+                ("kpos", C.c_void_p), ("vpos", C.c_void_p),
+                ("kview", C.c_void_p), ("k_nb1", C.c_int64), ("k_nb2", C.c_int64),
+                ("vview", C.c_void_p), ("v_nb1", C.c_int64), ("v_nb2", C.c_int64), ("n_kv", C.c_int),
+                ("mask", C.c_void_p), ("scale", C.c_float), ("softcap", C.c_float), ("dst", C.c_void_p)]
+
+
+def attn_program(q, k, v, dst, k_cache, v_cache, kpos, vpos, pos, n_head: int, n_head_kv: int, n_kv: int, scale: float, softcap: float = 0.0,
+                 mask=None, n_dims: int = 128, rope_mode: int = 0, freq_base: float = 10000.0, freq_scale: float = 1.0, ext_factor: float = 0.0,
+                 attn_factor: float = 1.0, beta_fast: float = 32.0, beta_slow: float = 1.0, n_ctx_orig: int = 0, freq_factors=None,
+                 qkv=None) -> int:
+    """One persistent-kernel launch of the decode attention phase (b200_attn_program); returns the planned nsplit.
+    k_cache / v_cache f16 [n_cells, n_head_kv, 128] (the K / V views are their first n_kv cells); kpos / vpos i64 [1], pos i32 [1]
+    on the device; mask f16 [n_kv] or None.  qkv = dict(types, ws:[3 weights], x, norm_w, eps) runs the q|k|v mat-vec in the
+    same launch, writing q, k, v as well."""
+    a = AttnArgs()
+    D = k_cache.shape[-1]
+    if qkv is not None:
+        for j in range(3):
+            a.type_qkv[j] = qkv["types"][j]; a.w_qkv[j] = qkv["ws"][j].data_ptr(); a.row_stride_qkv[j] = qkv["ws"][j].stride(0)
+        a.x = qkv["x"].data_ptr(); a.n_embd = qkv["x"].numel(); a.eps = qkv.get("eps", 1e-5)
+        a.norm_w = qkv["norm_w"].data_ptr() if qkv.get("norm_w") is not None else None
+    a.q, a.k, a.v, a.dst = q.data_ptr(), k.data_ptr(), v.data_ptr(), dst.data_ptr()
+    a.n_head, a.n_head_kv, a.head_dim, a.n_dims, a.rope_mode, a.n_ctx_orig = n_head, n_head_kv, D, n_dims, rope_mode, n_ctx_orig
+    a.freq_base, a.freq_scale, a.ext_factor, a.attn_factor, a.beta_fast, a.beta_slow = freq_base, freq_scale, ext_factor, attn_factor, beta_fast, beta_slow
+    a.freq_factors = freq_factors.data_ptr() if freq_factors is not None else None
+    a.pos = pos.data_ptr()
+    a.k_cache, a.k_row_bytes = k_cache.data_ptr(), k_cache.stride(0) * 2
+    a.v_cache, a.v_row_bytes = v_cache.data_ptr(), v_cache.stride(0) * 2
+    a.kpos, a.vpos = kpos.data_ptr(), vpos.data_ptr()
+    a.kview, a.k_nb1, a.k_nb2 = k_cache.data_ptr(), k_cache.stride(0) * 2, k_cache.stride(1) * 2
+    a.vview, a.v_nb1, a.v_nb2 = v_cache.data_ptr(), v_cache.stride(0) * 2, v_cache.stride(1) * 2
+    a.n_kv = n_kv
+    a.mask = mask.data_ptr() if mask is not None else None
+    a.scale, a.softcap = scale, softcap
+    ns = C.c_int(0)
+    _check(lib().b200_attn_program(C.byref(a), C.byref(ns), _stream()), "b200_attn_program")
+    return ns.value
 
 
 def mul_mat_id(t: int, w: torch.Tensor, b: torch.Tensor, ids: torch.Tensor) -> torch.Tensor:

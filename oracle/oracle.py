@@ -202,6 +202,184 @@ class Ref:
         assert rc == 0
         return out
 
+    # ---- one-node ggml graphs on the reference's CPU backend (ggml_init / ggml_new_tensor_4d / op / ggml_graph_compute_with_ctx)
+    def _graph_lib(self):
+        b, vp, i64 = self.base, C.c_void_p, C.c_int64
+        if getattr(self, "_graph_ready", False):
+            return b
+        b.ggml_init.restype = vp
+        b.ggml_init.argtypes = [_GgmlInitParams]
+        b.ggml_free.argtypes = [vp]
+        b.ggml_new_tensor_4d.restype = vp
+        b.ggml_new_tensor_4d.argtypes = [vp, C.c_int, i64, i64, i64, i64]
+        b.ggml_get_data.restype = vp
+        b.ggml_get_data.argtypes = [vp]
+        b.ggml_nbytes.restype = C.c_size_t
+        b.ggml_nbytes.argtypes = [vp]
+        b.ggml_flash_attn_ext.restype = vp
+        b.ggml_flash_attn_ext.argtypes = [vp, vp, vp, vp, vp, C.c_float, C.c_float, C.c_float]
+        b.ggml_rope_ext.restype = vp
+        b.ggml_rope_ext.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int] + [C.c_float] * 6
+        b.ggml_new_graph.restype = vp
+        b.ggml_new_graph.argtypes = [vp]
+        b.ggml_build_forward_expand.argtypes = [vp, vp]
+        self.cpu.ggml_graph_compute_with_ctx.restype = C.c_int
+        self.cpu.ggml_graph_compute_with_ctx.argtypes = [vp, vp, C.c_int]
+        self._graph_ready = True
+        return b
+
+    def _run_one_node(self, inputs, make_node, out_shape, mem: int):
+        """inputs: list of (ggml type, numpy array in ggml memory order, outermost first); make_node(ctx, tensors) -> node.
+        Returns the node's f32 data reshaped to out_shape."""
+        b = self._graph_lib()
+        ctx = b.ggml_init(_GgmlInitParams(mem + (64 << 20), None, False))
+        assert ctx
+        try:
+            ts = []
+            for typ, arr in inputs:
+                if arr is None:
+                    ts.append(None)
+                    continue
+                arr = np.ascontiguousarray(arr)
+                ne = list(arr.shape[::-1]) + [1] * (4 - arr.ndim)
+                t = b.ggml_new_tensor_4d(ctx, typ, *ne)
+                assert b.ggml_nbytes(t) == arr.nbytes
+                C.memmove(b.ggml_get_data(t), arr.ctypes.data, arr.nbytes)
+                ts.append(t)
+            node = make_node(ctx, ts)
+            gf = b.ggml_new_graph(ctx)
+            b.ggml_build_forward_expand(gf, node)
+            assert self.cpu.ggml_graph_compute_with_ctx(ctx, gf, 4) == 0
+            out = np.empty(out_shape, dtype=np.float32)
+            assert b.ggml_nbytes(node) == out.nbytes
+            C.memmove(out.ctypes.data, b.ggml_get_data(node), out.nbytes)
+            return out
+        finally:
+            b.ggml_free(ctx)
+
+    def flash_attn_ext(self, q, k, v, mask, scale: float, softcap: float = 0.0) -> np.ndarray:
+        """ggml_flash_attn_ext on the CPU backend.  Layouts as attention_f64 (q f32 [B, H, N, D], k / v f16 [B, Hkv, n_kv, D],
+        mask f16 [m3, m2, >= N, n_kv] or None); returns f32 [B, N, H, DV]."""
+        B, H, N, _ = q.shape
+        DV = v.shape[3]
+        ins = [(GGML_TYPE_F32, q.astype(np.float32)), (GGML_TYPE_F16, k.astype(np.float16)), (GGML_TYPE_F16, v.astype(np.float16)),
+               (GGML_TYPE_F16, None if mask is None else mask.astype(np.float16))]
+        mem = sum(a.nbytes for _, a in ins if a is not None) + B * N * H * DV * 4
+        return self._run_one_node(ins, lambda ctx, t: self.base.ggml_flash_attn_ext(ctx, t[0], t[1], t[2], t[3], scale, 0.0, softcap),
+                                  (B, N, H, DV), mem)
+
+    def rope_ext(self, x, pos, n_dims: int, mode: int, freq_base: float = 10000.0, freq_scale: float = 1.0, ext_factor: float = 0.0,
+                 attn_factor: float = 1.0, beta_fast: float = 32.0, beta_slow: float = 1.0, n_ctx_orig: int = 0, freq_factors=None) -> np.ndarray:
+        """ggml_rope_ext on the CPU backend: x f32 [T, H, D], pos i32 [T], freq_factors f32 [n_dims / 2] or None -> f32 [T, H, D]."""
+        x = np.asarray(x, dtype=np.float32)
+        ins = [(GGML_TYPE_F32, x), (26, np.asarray(pos, dtype=np.int32)),   # 26 = GGML_TYPE_I32
+               (GGML_TYPE_F32, None if freq_factors is None else np.asarray(freq_factors, dtype=np.float32))]
+        return self._run_one_node(ins, lambda ctx, t: self.base.ggml_rope_ext(ctx, t[0], t[1], t[2], n_dims, mode, n_ctx_orig, freq_base, freq_scale,
+                                                                                ext_factor, attn_factor, beta_fast, beta_slow),
+                                  x.shape, 2 * x.nbytes)
+
+
+_libm = C.CDLL("libm.so.6")
+_libm.powf.restype = _libm.logf.restype = C.c_float
+_libm.powf.argtypes = [C.c_float, C.c_float]
+_libm.logf.argtypes = [C.c_float]
+_f32 = np.float32
+
+
+def attention_f64(q, k, v, mask, scale: float, softcap: float = 0.0, want_abs: bool = False):
+    """FLASH_ATTN_EXT (ggml_compute_forward_flash_attn_ext_f16, ggml/src/ggml-cpu/ops.cpp) restated in float64.
+
+    Arrays are in ggml memory order, outermost dimension first: q f32 [B, H, N, DK], k / v f16 [Bk, Hkv, n_kv, D],
+    mask f16 [m3, m2, >= N, >= n_kv] or None.  Returns f64 [B, N, H, DV] (ggml dst [DV, H, N, B]) and, with want_abs, also
+    A[b, n, h, d] = sum_j p_j |v_jd| / sum_j p_j, the scale a per-element error bound is taken relative to.
+
+    q is rounded to f16 first (K is f16); s = scale * q.k, with softcap: softcap * tanh(s) where scale was divided by softcap
+    beforehand (in f32, as ggml does); then + mask.  Keys whose mask is -inf are skipped; a row with no key left gives 0.
+    Head h reads kv head h / (H / Hkv), batch b reads b / (B / Bk), the mask plane (h % m2, b % m3)."""
+    B, H, N, DK = q.shape
+    Bk, Hkv, n_kv, _ = k.shape
+    DV = v.shape[3]
+    sc = float(_f32(scale) / _f32(softcap)) if softcap != 0.0 else float(scale)
+    out = np.zeros((B, N, H, DV))
+    A = np.zeros((B, N, H, DV)) if want_abs else None
+    q16 = q.astype(np.float16).astype(np.float64)
+    g, gb = H // Hkv, B // Bk
+    for b in range(B):
+        for hk in range(Hkv):
+            kk = k[b // gb, hk].astype(np.float64)
+            vv = v[b // (B // v.shape[0]), hk].astype(np.float64)
+            hs = range(hk * g, (hk + 1) * g)
+            s = (q16[b, hk * g:(hk + 1) * g] @ kk.T) * sc
+            if softcap != 0.0:
+                s = softcap * np.tanh(s)
+            if mask is not None:
+                m = np.stack([mask[b % mask.shape[0], h % mask.shape[1], :N, :n_kv] for h in hs]).astype(np.float64)
+                s = s + m
+            live = s != -np.inf
+            smax = np.where(live, s, -np.inf).max(-1, keepdims=True)
+            p = np.where(live, np.exp(s - np.where(np.isfinite(smax), smax, 0.0)), 0.0)
+            l = p.sum(-1, keepdims=True)
+            inv = np.where(l > 0, 1.0 / np.where(l > 0, l, 1.0), 0.0)
+            out[b, :, hk * g:(hk + 1) * g] = ((p @ vv) * inv).transpose(1, 0, 2)
+            if want_abs:
+                A[b, :, hk * g:(hk + 1) * g] = ((p @ np.abs(vv)) * inv).transpose(1, 0, 2)
+    return (out, A) if want_abs else out
+
+
+def rope_theta_scale(freq_base: float, n_dims: int) -> np.float32:
+    """powf(freq_base, -2.0f / n_dims) with the C library's powf, as ggml computes it on the host."""
+    return _f32(_libm.powf(float(freq_base), float(_f32(-2.0) / _f32(n_dims))))
+
+
+def rope_corr_dims(n_dims: int, n_ctx_orig: int, freq_base: float, beta_fast: float, beta_slow: float):
+    """ggml_rope_yarn_corr_dims (ggml/src/ggml.c) in f32."""
+    def dim(n_rot):
+        num = _f32(_libm.logf(float(_f32(n_ctx_orig) / (_f32(n_rot) * _f32(2) * _f32(np.pi)))))
+        return _f32(_f32(n_dims) * num) / _f32(_f32(2) * _f32(_libm.logf(float(freq_base))))
+    start, end = np.floor(dim(beta_fast)), np.ceil(dim(beta_slow))
+    return _f32(max(0.0, start)), _f32(min(n_dims - 1, end))
+
+
+def rope_ref(x, pos, n_dims: int, mode: int, freq_base: float = 10000.0, freq_scale: float = 1.0, ext_factor: float = 0.0,
+             attn_factor: float = 1.0, beta_fast: float = 32.0, beta_slow: float = 1.0, n_ctx_orig: int = 0, freq_factors=None):
+    """ROPE (ggml_compute_forward_rope, modes 0 and 2 = NEOX) of x f32 [T, H, D] (ggml [D, H, T]) at positions pos i32 [T].
+
+    theta is iterated in f32 exactly as ggml_rope_cache_init does (theta *= theta_scale per pair, divided by the pair's
+    freq_factor, YaRN ramp and interpolation in f32); cos / sin and the rotation are then taken in float64.  Dims >= n_dims
+    pass through.  Returns f64 [T, H, D]."""
+    x = np.asarray(x, dtype=np.float32)
+    T, H, D = x.shape
+    half = n_dims // 2
+    ts = rope_theta_scale(freq_base, n_dims)
+    corr0, corr1 = rope_corr_dims(n_dims, n_ctx_orig, freq_base, beta_fast, beta_slow)
+    fs, ef = _f32(freq_scale), _f32(ext_factor)
+    mscale = _f32(attn_factor)
+    if ef != 0:
+        mscale = _f32(mscale * _f32(_f32(1) + _f32(0.1) * _f32(_libm.logf(float(_f32(1) / fs)))))
+    out = x.astype(np.float64).copy()
+    for t in range(T):
+        theta = _f32(pos[t])
+        for i in range(half):
+            ff = _f32(freq_factors[i]) if freq_factors is not None else _f32(1)
+            th_ex = _f32(theta / ff)
+            th_in = _f32(fs * th_ex)
+            th = th_in
+            if ef != 0:
+                y = _f32(_f32(_f32(i) - corr0) /_f32(max(_f32(0.001), _f32(corr1 - corr0))))
+                ramp = _f32(_f32(1 - min(_f32(1), max(_f32(0), y))) * ef)
+                th = _f32(_f32(th_in * _f32(1 - ramp)) + _f32(th_ex * ramp))
+            c, s = np.cos(np.float64(th)) * float(mscale), np.sin(np.float64(th)) * float(mscale)
+            ia, ib = (2 * i, 2 * i + 1) if mode == 0 else (i, i + half)
+            x0, x1 = x[t, :, ia].astype(np.float64), x[t, :, ib].astype(np.float64)
+            out[t, :, ia] = x0 * c - x1 * s
+            out[t, :, ib] = x0 * s + x1 * c
+            theta = _f32(theta * ts)
+    return out
+
+
+class _GgmlInitParams(C.Structure):
+    _fields_ = [("mem_size", C.c_size_t), ("mem_buffer", C.c_void_p), ("no_alloc", C.c_bool)]
+
 
 def random_blocks(t: int, rows: int, k: int, rng: np.random.Generator, scale: float = 0.02) -> np.ndarray:
     """Random but VALID quantised rows (uint8 [rows, row_bytes]) without running a quantiser:

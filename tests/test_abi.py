@@ -30,6 +30,13 @@ def test_every_declared_symbol_is_exported(lib):
         assert hasattr(lib, s), f"{s} declared in include/b200_qmm.h but not exported by libb200qmm.so"
 
 
+def test_every_attention_symbol_is_exported(lib):
+    syms = declared_symbols("b200_attn.h")
+    assert syms == ["b200_attn_program", "b200_flash_attn", "b200_flash_attn_workspace_bytes"]
+    for s in syms:
+        assert hasattr(lib, s), f"{s} declared in include/b200_attn.h but not exported by libb200qmm.so"
+
+
 def test_plugin_exports_every_symbol_its_header_declares():
     """libggml-b200.so (the drop-in boundary): the two dl entry points + the bench hooks of include/ggml-b200.h, and the
     kernel C ABI it embeds.  Symbol table only -- loading it needs libggml-base and calling it needs a GPU."""
@@ -44,7 +51,7 @@ def test_plugin_exports_every_symbol_its_header_declares():
     assert {"ggml_backend_init", "ggml_backend_score"} <= declared
     for s in sorted(declared):
         assert s in exported, f"{s} declared in include/ggml-b200.h but not exported by libggml-b200.so"
-    for s in declared_symbols("b200_qmm.h"):
+    for s in declared_symbols("b200_qmm.h") + declared_symbols("b200_attn.h"):
         assert s in exported, s
 
 
@@ -111,3 +118,40 @@ def test_sass_has_no_local_memory_in_gemv():
     assert len(hot) == 5
     for name, stack, st, ld in hot:
         assert int(st) == 0 and int(ld) == 0 and int(stack) == 0, (name, stack, st, ld)
+
+
+def test_attention_arguments_fail_before_touching_the_gpu(lib):
+    """b200_flash_attn / b200_attn_program reject unsupported or inconsistent shapes on the host (no device memory is named)."""
+    lib.b200_qmm_last_error.restype = C.c_char_p
+    I4 = C.c_int64 * 4
+    vp = C.c_void_p
+    lib.b200_flash_attn.argtypes = [vp, C.POINTER(C.c_int64), C.POINTER(C.c_int64)] * 5 + [C.c_float, C.c_float, vp, C.c_size_t, C.c_int, vp]
+
+    def fa(D, N, H, Hkv, path, n_kv=64):
+        q_ne, k_ne, d_ne = I4(D, N, H, 1), I4(D, n_kv, Hkv, 1), I4(D, H, N, 1)
+        q_nb, k_nb, d_nb = I4(4, 4 * D, 4 * D * N, 4 * D * N * H), I4(2, 2 * D, 2 * D * n_kv, 2 * D * n_kv * Hkv), I4(4, 4 * D, 4 * D * H, 4 * D * H * N)
+        return lib.b200_flash_attn(None, q_ne, q_nb, None, k_ne, k_nb, None, k_ne, k_nb, None, None, None, None, d_ne, d_nb,
+                                   0.1, 0.0, None, 0, path, None)
+
+    assert fa(96, 32, 4, 4, 2) == -6                         # the tensor-core kernel: D in {64, 128} only, no fall-back
+    assert b"tensor-core" in lib.b200_qmm_last_error()
+    assert fa(256, 32, 4, 4, 2) == -6
+    assert fa(128, 15, 4, 4, 2) == -6                        # ... and >= 16 rows
+    assert fa(320, 1, 4, 4, 1) == -6                         # the scalar kernel: D <= 256
+    assert fa(128, 4, 6, 4, 1) == -1                         # H not a multiple of Hkv
+    assert fa(128, 4, 4, 4, 3) == -1                         # unknown path
+
+    class Args(C.Structure):                                  # the leading fields of b200_attn_args, the rest zero
+        _fields_ = [("type_qkv", C.c_int * 3), ("w_qkv", vp * 3), ("row_stride_qkv", C.c_int64 * 3), ("x", vp), ("norm_w", vp),
+                    ("n_embd", C.c_int64), ("eps", C.c_float), ("q", vp), ("k", vp), ("v", vp),
+                    ("n_head", C.c_int), ("n_head_kv", C.c_int), ("head_dim", C.c_int), ("n_dims", C.c_int), ("rope_mode", C.c_int),
+                    ("pad", C.c_char * 512)]
+
+    lib.b200_attn_program.argtypes = [C.POINTER(Args), C.POINTER(C.c_int), vp]
+    a = Args(n_head=32, n_head_kv=8, head_dim=64, n_dims=64)
+    assert lib.b200_attn_program(C.byref(a), None, None) == -6   # head_dim != 128
+    assert b"head_dim" in lib.b200_qmm_last_error()
+    a = Args(n_head=32, n_head_kv=6, head_dim=128, n_dims=128)
+    assert lib.b200_attn_program(C.byref(a), None, None) == -1   # n_head not a multiple of n_head_kv
+    assert b"n_head_kv" in lib.b200_qmm_last_error()
+    assert lib.b200_attn_program(None, None, None) == -1

@@ -148,3 +148,93 @@ def test_empty_and_sizes(oracle):
         assert oracle.lib.orc_dequantize_row(t, None, None, 0) == 0
         assert oracle.lib.orc_dequantize_row(t, None, None, BLOCK_ELEMS[t] + 1) == -1  # ragged K is rejected, as ggml asserts
         assert oracle.lib.orc_row_bytes(t, 4096) == 4096 // BLOCK_ELEMS[t] * BLOCK_BYTES[t]
+
+
+# ---- attention and ROPE: the float64 restatements the GPU attention tests compare against, pinned to ggml's own CPU code
+
+def _fa_case(rng, B, H, Hkv, N, n_kv, D, mask_kind):
+    q = rng.standard_normal((B, H, N, D)).astype(np.float32)
+    k = rng.standard_normal((B, Hkv, n_kv, D)).astype(np.float16)
+    v = rng.standard_normal((B, Hkv, n_kv, D)).astype(np.float16)
+    if mask_kind is None:
+        return q, k, v, None
+    m2 = H if mask_kind == "per_head" else 1
+    m = np.where(rng.random((B, m2, N, n_kv)) < 0.3, -np.inf, rng.uniform(-2, 2, (B, m2, N, n_kv))).astype(np.float16)
+    m[:, :, 1, :] = -np.inf                                   # a row with every key masked: 0, not NaN
+    return q, k, v, m
+
+
+@pytest.mark.parametrize("B,H,Hkv,N,n_kv,D,mask_kind,softcap", [
+    (1, 4, 4, 3, 17, 64, None, 0.0),
+    (2, 8, 2, 5, 37, 64, "broadcast", 0.0),                   # GQA 4, one mask plane for every head
+    (1, 8, 1, 4, 70, 128, "per_head", 0.0),                   # GQA 8, mask ne2 = H
+    (2, 4, 2, 6, 129, 128, "broadcast", 30.0),                # softcap
+    (1, 2, 1, 2, 300, 256, "per_head", 0.0),
+])
+def test_attention_f64_matches_ggml_cpu_flash_attn(ref, B, H, Hkv, N, n_kv, D, mask_kind, softcap):
+    """The restatement against ggml_flash_attn_ext on the reference's CPU backend, which accumulates V in f16: <= 2e-3 max|v|."""
+    from oracle.oracle import attention_f64
+    rng = np.random.default_rng(N * 1000 + n_kv)
+    q, k, v, m = _fa_case(rng, B, H, Hkv, N, n_kv, D, mask_kind)
+    scale = 1.0 / np.sqrt(D)
+    want = ref.flash_attn_ext(q, k, v, m, scale, softcap)
+    got = attention_f64(q, k, v, m, scale, softcap)
+    assert np.isfinite(want).all() and np.isfinite(got).all()
+    assert np.abs(got - want).max() <= 2e-3 * np.abs(v.astype(np.float32)).max()
+    if m is not None:
+        assert (got[:, 1] == 0).all() and (want[:, 1] == 0).all()
+
+
+def test_attention_f64_semantics():
+    """GQA head mapping, K/V broadcast over the batch, softcap and peaked scores, on a case small enough to state by hand."""
+    from oracle.oracle import attention_f64
+    rng = np.random.default_rng(3)
+    q = rng.standard_normal((2, 4, 3, 32)).astype(np.float32)
+    k = rng.standard_normal((1, 2, 5, 32)).astype(np.float16)
+    v = rng.standard_normal((1, 2, 5, 32)).astype(np.float16)
+    got = attention_f64(q, k, v, None, 0.3, 0.0)
+    for b in range(2):
+        for h in range(4):
+            s = 0.3 * q[b, h].astype(np.float16).astype(np.float64) @ k[0, h // 2].astype(np.float64).T
+            p = np.exp(s - s.max(-1, keepdims=True))
+            assert np.allclose(got[b, :, h], (p / p.sum(-1, keepdims=True)) @ v[0, h // 2].astype(np.float64), rtol=0, atol=1e-12)
+    capped = attention_f64(q * 100, k, v, None, 0.3, 5.0)
+    s = 5.0 * np.tanh(float(np.float32(0.3) / np.float32(5.0)) * (q[0, 0] * 100).astype(np.float16).astype(np.float64) @ k[0, 0].astype(np.float64).T)
+    p = np.exp(s - s.max(-1, keepdims=True))
+    assert np.allclose(capped[0, :, 0], (p / p.sum(-1, keepdims=True)) @ v[0, 0].astype(np.float64), rtol=0, atol=1e-12)
+
+
+@pytest.mark.parametrize("kw,pos", [
+    (dict(n_dims=128, mode=0), [0, 1, 7, 4095, 100000]),
+    (dict(n_dims=128, mode=2), [0, 3, 100000]),
+    (dict(n_dims=64, mode=0), [5, 77777]),                                            # dims 64..127 pass through
+    (dict(n_dims=64, mode=2, with_ff=True, freq_base=500000.0), [9, 100000]),         # freq_factors (Llama 3)
+    (dict(n_dims=128, mode=0, ext_factor=1.0, freq_scale=0.25, n_ctx_orig=4096, attn_factor=1.0), [0, 5, 300]),   # YaRN ramp + mscale
+    (dict(n_dims=128, mode=2, ext_factor=0.5, freq_scale=0.5, n_ctx_orig=2048, beta_fast=16.0, beta_slow=2.0), [1, 60]),
+])
+def test_rope_ref_matches_ggml_cpu_rope(ref, kw, pos):
+    """rope_ref against ggml_rope_ext on the reference's CPU backend: within 8 f32 ulps of |x0| + |x1| of each pair (times
+    mscale).  (YaRN at large positions is left out: where the ramp mixes the two thetas, ggml's f32 expression may be
+    contracted into an FMA, which moves theta by an ulp -- 1e-2 rad at pos 1e5.)"""
+    from oracle.oracle import rope_ref
+    kw = dict(kw)
+    rng = np.random.default_rng(len(pos) + kw["n_dims"])
+    if kw.pop("with_ff", False):
+        kw["freq_factors"] = rng.uniform(1.0, 8.0, kw["n_dims"] // 2).astype(np.float32)
+    x = rng.standard_normal((len(pos), 6, 128)).astype(np.float32)
+    p = np.array(pos, dtype=np.int32)
+    want = ref.rope_ext(x, p, **kw)
+    got = rope_ref(x, p, **kw)
+    nd = kw["n_dims"]
+    pair = np.abs(x).copy()
+    if kw["mode"] == 0:
+        pair[..., 0:nd:2] = pair[..., 1:nd:2] = np.abs(x[..., 0:nd:2]) + np.abs(x[..., 1:nd:2])
+    else:
+        pair[..., :nd // 2] = pair[..., nd // 2:nd] = np.abs(x[..., :nd // 2]) + np.abs(x[..., nd // 2:nd])
+    mscale = 1.0 + (0.1 * np.log(1.0 / kw["freq_scale"]) if kw.get("ext_factor", 0.0) else 0.0)
+    bound = 8 * 2.0 ** -24 * pair * mscale * kw.get("attn_factor", 1.0)
+    err = np.abs(got - want)
+    assert (err <= bound).all(), float((err / bound).max())
+    assert np.array_equal(got[..., nd:], x[..., nd:].astype(np.float64))
+    if pos[0] == 0 and not kw.get("ext_factor"):
+        assert np.array_equal(got[0], x[0].astype(np.float64))   # pos 0: ROPE is exactly the identity
