@@ -1,4 +1,4 @@
-// c_abi.cu -- the extern "C" surface declared in include/b200_qmm.h and include/b200_attn.h.  Thin: argument checks, workspace carving,
+// c_abi.cu -- the extern "C" surface declared in include/b200_qmm.h, include/b200_attn.h and include/b200_moe.h.  Thin: argument checks, workspace carving,
 // regime selection (decode GEMV vs prefill GEMM), error text.  No compute happens on the host and there is no CPU
 // fallback: if CUDA is unusable every compute entry point fails loudly.
 #include <atomic>
@@ -8,12 +8,14 @@
 
 #include "../../include/b200_qmm.h"
 #include "../../include/b200_attn.h"
+#include "../../include/b200_moe.h"
 #include "qmm_formats.cuh"
 #include <vector>
 #include <string.h>
 #include "qmm_kernels.cuh"
 #include "qmm_ops.cuh"
 #include "qmm_attn.cuh"
+#include "qmm_moe.cuh"
 #include "decode_flow.cuh"
 
 namespace qmm {
@@ -351,18 +353,14 @@ size_t b200_mul_mat_id_workspace_bytes(int type, int64_t M, int64_t K, int64_t n
     return type_ok(type) ? act_workspace_bytes(type, nb1 * T, K) + 256 : 0;
 }
 
-int b200_mul_mat_id(int type, const void * w, int64_t row_stride, int64_t expert_stride, int64_t n_expert, int64_t M, int64_t K,
-                    const float * b, int64_t nb1, const int32_t * ids, int64_t ids_stride, int64_t n_used, int64_t T,
-                    float * dst, void * ws, size_t ws_bytes, void * stream) {
-    if (!type_ok(type) || M < 0 || T < 0 || n_used <= 0 || n_expert <= 0 || K <= 0 || K % block_elems(type) || (nb1 != 1 && nb1 != n_used))
-        return fail(B200_E_INVALID, "b200_mul_mat_id: bad type/shape");
-    if (M == 0 || T == 0) return B200_OK;
-    if (ws_bytes < b200_mul_mat_id_workspace_bytes(type, M, K, n_used, T, nb1)) return fail(B200_E_WORKSPACE, "b200_mul_mat_id: workspace too small");
-    cudaStream_t st = (cudaStream_t)stream;
+// The routed GEMV over all (token, slot) rows, in token chunks: gridDim.y = chunk * n_used <= 65535.  As b200_mul_mat_id below and
+// the backend's run_mul_mat_id do it.
+static cudaError_t mul_mat_id_gemv(int type, const void * w, int64_t row_stride, int64_t expert_stride, int64_t n_expert, int64_t M, int64_t K,
+                                   const float * b, int64_t nb1, const int32_t * ids, int64_t ids_stride, int64_t n_used, int64_t T,
+                                   float * dst, void * ws, cudaStream_t st) {
     const ActQ8 act = act_carve(type, ws, nb1 * T, K);
     cudaError_t e = launch_quantize_act(type, b, K, nb1 * T, K, act, st);
-    if (e != cudaSuccess) return from_cuda(e, "b200_mul_mat_id(quantize)");
-    // gridDim.y <= 65535: chunk the (slot, token) pairs by whole tokens
+    if (e != cudaSuccess) return e;
     const int64_t t_chunk = 65535 / n_used;
     for (int64_t t0 = 0; t0 < T; t0 += t_chunk) {
         const int64_t nt = T - t0 < t_chunk ? T - t0 : t_chunk;
@@ -373,9 +371,82 @@ int b200_mul_mat_id(int type, const void * w, int64_t row_stride, int64_t expert
         a.dst = dst + t0 * n_used * M; a.ldd = M; a.residual = nullptr;
         a.ids = ids + t0 * ids_stride; a.ids_stride = ids_stride; a.n_used = (int)n_used; a.nb1 = (int)nb1; a.n_expert = (int)n_expert;
         e = launch_gemv(type, a, st);
-        if (e != cudaSuccess) return from_cuda(e, "b200_mul_mat_id(gemv)");
+        if (e != cudaSuccess) return e;
     }
-    return B200_OK;
+    return cudaSuccess;
+}
+
+size_t b200_mul_mat_id_path_workspace_bytes(int type, int64_t M, int64_t K, int64_t n_expert, int64_t n_used, int64_t T, int64_t nb1) {
+    if (!type_ok(type)) return 0;
+    const size_t a = act_workspace_bytes(type, nb1 * T, K);
+    const size_t g = gemm_grouped_workspace_bytes(type, M, n_used * T, n_expert, K);
+    return (a > g ? a : g) + 256;
+}
+
+int b200_mul_mat_id_path(int type, const void * w, int64_t row_stride, int64_t expert_stride, int64_t n_expert, int64_t M, int64_t K,
+                         const float * b, int64_t nb1, const int32_t * ids, int64_t ids_stride, int64_t n_used, int64_t T,
+                         float * dst, void * ws, size_t ws_bytes, int path, int * taken, void * stream) {
+    if (taken) *taken = 0;
+    if (path < 0 || path > 2) return fail(B200_E_INVALID, "b200_mul_mat_id_path: path must be 0, 1 or 2");
+    if (!type_ok(type) || M < 0 || T < 0 || n_used <= 0 || n_expert <= 0 || K <= 0 || K % block_elems(type) || (nb1 != 1 && nb1 != n_used))
+        return fail(B200_E_INVALID, "b200_mul_mat_id_path: bad type/shape (n_used > 0, nb1 in {1, n_used})");
+    if (M > INT32_MAX || K > INT32_MAX || T * n_used > INT32_MAX || n_expert > INT32_MAX) return fail(B200_E_INVALID, "b200_mul_mat_id_path: dimension too large");
+    if (M == 0 || T == 0) return B200_OK;
+    if (ws_bytes < b200_mul_mat_id_path_workspace_bytes(type, M, K, n_expert, n_used, T, nb1))
+        return fail(B200_E_WORKSPACE, "b200_mul_mat_id_path: workspace too small");
+    cudaStream_t st = (cudaStream_t)stream;
+    // path 0 restates the rule of run_mul_mat_id (backend/ggml_b200.cpp), which the plugin's prebuilt objects compile in: keep the two
+    // in step.  Many (token, slot) rows and a grouped workspace (K-quant, n_expert <= 256) take the grouped GEMM; operands it cannot
+    // take fall back to the GEMV.
+    const int64_t jobs = T * n_used;
+    if (path == 2 || (path == 0 && jobs >= 32 && gemm_grouped_workspace_bytes(type, M, jobs, n_expert, K) != 0)) {
+        GemmGroupedArgs ga{};
+        ga.w = (const uint8_t *)w; ga.row_stride = row_stride; ga.expert_stride = expert_stride; ga.M = (int)M; ga.K = (int)K; ga.n_expert = (int)n_expert;
+        ga.x = b; ga.ldx = K; ga.nb1 = (int)nb1;
+        ga.ids = ids; ga.ids_stride = ids_stride; ga.T = (int)T; ga.n_used = (int)n_used;
+        ga.dst = dst; ga.ldd = M; ga.workspace = ws; ga.workspace_bytes = ws_bytes;
+        const cudaError_t ge = launch_gemm_grouped(type, ga, st);
+        if (ge == cudaErrorNotSupported || ge == cudaErrorMisalignedAddress) {
+            cudaGetLastError();
+            if (path == 2) return fail(B200_E_UNSUPPORTED, "b200_mul_mat_id_path: the grouped GEMM takes K-quant experts, n_expert <= 256 and aligned operands");
+        } else {
+            if (ge == cudaSuccess && taken) *taken = 2;
+            return from_cuda(ge, "b200_mul_mat_id_path(grouped gemm)");
+        }
+    }
+    const cudaError_t e = mul_mat_id_gemv(type, w, row_stride, expert_stride, n_expert, M, K, b, nb1, ids, ids_stride, n_used, T, dst, ws, st);
+    if (e == cudaSuccess && taken) *taken = 1;
+    return from_cuda(e, "b200_mul_mat_id_path(gemv)");
+}
+
+int64_t b200_moe_route_max_tiles(int64_t n_expert, int64_t n_used, int64_t T) {
+    if (n_expert <= 0 || n_used <= 0 || T < 0) return 0;
+    return moe_max_tiles(T * n_used, n_expert);
+}
+
+int64_t b200_moe_route(const int32_t * ids, int64_t ids_stride, int64_t n_expert, int64_t n_used, int64_t T, int64_t nb1,
+                       int32_t * tile_expert, int32_t * col_src, int32_t * col_dst, void * stream) {
+    if (n_used <= 0 || T <= 0 || n_expert <= 0 || (nb1 != 1 && nb1 != n_used) || !ids || !tile_expert || !col_src || !col_dst)
+        return fail(B200_E_INVALID, "b200_moe_route: bad arguments (n_used > 0, T > 0, nb1 in {1, n_used})");
+    if (n_expert > 256) return fail(B200_E_UNSUPPORTED, "b200_moe_route: n_expert must be <= 256");
+    const int64_t max_tiles = moe_max_tiles(T * n_used, n_expert);
+    if (T * n_used > INT32_MAX || max_tiles * MOE_TILE_COLS > INT32_MAX) return fail(B200_E_INVALID, "b200_moe_route: too many jobs");
+    note_launch();
+    const cudaError_t e = launch_moe_route(ids, ids_stride, (int)T, (int)n_used, (int)nb1, (int)n_expert, (int)max_tiles, tile_expert, col_src, col_dst,
+                                           (cudaStream_t)stream);
+    if (e != cudaSuccess) return from_cuda(e, "b200_moe_route");
+    return max_tiles;
+}
+
+int b200_mul_mat_id(int type, const void * w, int64_t row_stride, int64_t expert_stride, int64_t n_expert, int64_t M, int64_t K,
+                    const float * b, int64_t nb1, const int32_t * ids, int64_t ids_stride, int64_t n_used, int64_t T,
+                    float * dst, void * ws, size_t ws_bytes, void * stream) {
+    if (!type_ok(type) || M < 0 || T < 0 || n_used <= 0 || n_expert <= 0 || K <= 0 || K % block_elems(type) || (nb1 != 1 && nb1 != n_used))
+        return fail(B200_E_INVALID, "b200_mul_mat_id: bad type/shape");
+    if (M == 0 || T == 0) return B200_OK;
+    if (ws_bytes < b200_mul_mat_id_workspace_bytes(type, M, K, n_used, T, nb1)) return fail(B200_E_WORKSPACE, "b200_mul_mat_id: workspace too small");
+    return from_cuda(mul_mat_id_gemv(type, w, row_stride, expert_stride, n_expert, M, K, b, nb1, ids, ids_stride, n_used, T, dst, ws, (cudaStream_t)stream),
+                     "b200_mul_mat_id");
 }
 
 size_t b200_mul_mat_host_scratch_bytes(int type, int64_t M, int64_t N, int64_t K) {

@@ -8,7 +8,9 @@
 //   integers, exactly representable in fp16:
 //       A  = sc_j * q_w      (<= 63*15 for Q4_K, 63*31 for Q5_K)      B  = q_a (the CPU-identical Q8_K integers)
 //       A' = m_j             (6 bit)                                    B' = bsum_j split into (even part, low bit)
-//   wgmma.mma_async accumulates them in fp32 registers (exact below 2^24).  After every K block the block's integer sums are
+//   wgmma.mma_async accumulates them in fp32 registers: exact while a block's partial sums stay below 2^24, which a saturated
+//   block exceeds (main sum up to 256*63*15*127 ~ 3.1e7 for Q4_K, 6.3e7 Q5_K, 1.3e8 Q6_K); there the fp32 rounding keeps the
+//   result within 6e-6 * sum |w x| (worst 0.21 of that measured on an H100 SXM at 700 W, DESIGN.md 3).  After every K block the block's integer sums are
 //   combined in registers with the block's fp16/fp32 scales:
 //       acc += (d_w d_a) * main - (dmin_w d_a) * mins
 //   i.e. the same per-block fp32 combine the CPU does (the mins term is added first).
@@ -26,6 +28,7 @@
 #include "gemm_layout.cuh"
 #include "qmm_formats.cuh"
 #include "qmm_kernels.cuh"
+#include "qmm_moe.cuh"
 #include "tcgen05_ptx.cuh"
 
 namespace qmm {
@@ -489,11 +492,20 @@ __global__ void __launch_bounds__(1024) moe_route_kernel(const int32_t * __restr
     }
 }
 
+static_assert(MOE_TILE_COLS == GEMM_NT, "the router's tiles are the GEMM's column tiles");
+
+cudaError_t launch_moe_route(const int32_t * ids, int64_t ids_stride, int T, int n_used, int nb1, int n_expert, int max_tiles,
+                             int * tile_expert, int * col_src, int * col_dst, cudaStream_t st) {
+    if (n_expert <= 0 || n_expert > 256) return cudaErrorNotSupported;      // the per-expert counters live in shared memory
+    moe_route_kernel<<<1, 1024, 0, st>>>(ids, ids_stride, T, n_used, nb1, n_expert, GEMM_NT, max_tiles, tile_expert, col_src, col_dst);
+    return cudaGetLastError();
+}
+
 size_t gemm_grouped_workspace_bytes(int type, int64_t M, int64_t jobs, int64_t n_expert, int64_t K) {
     (void)M;
     if (!(type == T_Q4_K || type == T_Q5_K || type == T_Q6_K) || K % 256 || jobs <= 0 || n_expert > 256) return 0;
     const int NT = GEMM_NT;
-    const int64_t max_tiles = (jobs + NT - 1) / NT + n_expert, nkb = K / 256;
+    const int64_t max_tiles = moe_max_tiles(jobs, n_expert), nkb = K / 256;
     return (size_t)(max_tiles * nkb * gl::bimg_block_bytes(NT) + nkb * max_tiles * NT * 4 + (max_tiles + 2 * max_tiles * NT) * 4 + 2048);
 }
 
@@ -503,15 +515,14 @@ cudaError_t launch_gemm_grouped(int type, const GemmGroupedArgs & a, cudaStream_
     if ((reinterpret_cast<uintptr_t>(a.x) & 15) || (a.ldx & 3)) return cudaErrorMisalignedAddress;
     const int NT = GEMM_NT;
     const int64_t jobs = (int64_t)a.T * a.n_used;
-    const int max_tiles = (int)((jobs + NT - 1) / NT + a.n_expert), nkb = a.K / 256, npad = max_tiles * NT;
+    const int max_tiles = (int)moe_max_tiles(jobs, a.n_expert), nkb = a.K / 256, npad = max_tiles * NT;
     if (a.workspace_bytes < gemm_grouped_workspace_bytes(type, a.M, jobs, a.n_expert, a.K)) return cudaErrorInvalidValue;
     uint8_t * bimg = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(a.workspace) + 255) & ~uintptr_t(255));
     float * da = reinterpret_cast<float *>(bimg + (int64_t)max_tiles * nkb * gl::bimg_block_bytes(NT));
     int * tile_expert = reinterpret_cast<int *>(da + (int64_t)nkb * npad);
     int * col_src = tile_expert + max_tiles, * col_dst = col_src + npad;
     note_launch(2);
-    moe_route_kernel<<<1, 1024, 0, st>>>(a.ids, a.ids_stride, a.T, a.n_used, a.nb1, a.n_expert, NT, max_tiles, tile_expert, col_src, col_dst);
-    cudaError_t e = cudaGetLastError();
+    cudaError_t e = launch_moe_route(a.ids, a.ids_stride, a.T, a.n_used, a.nb1, a.n_expert, max_tiles, tile_expert, col_src, col_dst, st);
     if (e != cudaSuccess) return e;
     quantize_act_gemm_kernel<<<dim3((unsigned)nkb, (unsigned)(npad / 8)), 256, 0, st>>>(a.x, a.ldx, 0, nkb, npad, bimg, da, NT, col_src);
     e = cudaGetLastError();

@@ -52,6 +52,13 @@ def lib() -> C.CDLL:
         L.b200_mul_mat_id_workspace_bytes.restype = sz
         L.b200_mul_mat_id_workspace_bytes.argtypes = [ci, i64, i64, i64, i64, i64]
         L.b200_mul_mat_id.argtypes = [ci, vp, i64, i64, i64, i64, i64, vp, i64, vp, i64, i64, i64, vp, vp, sz, vp]
+        L.b200_mul_mat_id_path_workspace_bytes.restype = sz
+        L.b200_mul_mat_id_path_workspace_bytes.argtypes = [ci, i64, i64, i64, i64, i64, i64]
+        L.b200_mul_mat_id_path.argtypes = [ci, vp, i64, i64, i64, i64, i64, vp, i64, vp, i64, i64, i64, vp, vp, sz, ci, C.POINTER(ci), vp]
+        L.b200_moe_route_max_tiles.restype = i64
+        L.b200_moe_route_max_tiles.argtypes = [i64, i64, i64]
+        L.b200_moe_route.restype = i64
+        L.b200_moe_route.argtypes = [vp, i64, i64, i64, i64, i64, vp, vp, vp, vp]
         L.b200_mul_mat_host_scratch_bytes.restype = sz
         L.b200_mul_mat_host_scratch_bytes.argtypes = [ci, i64, i64, i64]
         L.b200_mul_mat_host.argtypes = [ci, vp, i64, i64, i64, vp, i64, vp, vp, sz, vp]
@@ -263,19 +270,47 @@ def attn_program(q, k, v, dst, k_cache, v_cache, kpos, vpos, pos, n_head: int, n
     return ns.value
 
 
-def mul_mat_id(t: int, w: torch.Tensor, b: torch.Tensor, ids: torch.Tensor) -> torch.Tensor:
-    """w uint8 [E, M, row_bytes]; b f32 [T, nb1, K]; ids int32 [T, n_used] (row-strided ok) -> f32 [T, n_used, M]."""
+def mul_mat_id(t: int, w: torch.Tensor, b: torch.Tensor, ids: torch.Tensor, path: int | None = None, out: torch.Tensor | None = None):
+    """w uint8 [E, M, row_bytes]; b f32 [T, nb1, K]; ids int32 [T, n_used] (any row stride, e.g. the first n_used columns of an
+    [T, n_expert] argsort) -> f32 [T, n_used, M].
+    path None: b200_mul_mat_id (the routed GEMV), returns out.  path 0 / 1 / 2: b200_mul_mat_id_path (0 the backend's choice, 1 the
+    routed GEMV, 2 the grouped GEMM), returns (out, the kernel taken: 1 GEMV, 2 grouped GEMM).  out: the dst tensor to write."""
     E, M, rb = w.shape
     T, nb1, K = b.shape
     n_used = ids.shape[1]
     assert b.is_contiguous() and ids.dtype == torch.int32 and ids.stride(1) == 1
     L = lib()
-    out = torch.empty((T, n_used, M), dtype=torch.float32, device=b.device)
-    need = L.b200_mul_mat_id_workspace_bytes(t, M, K, n_used, T, nb1)
+    if out is None:
+        out = torch.empty((T, n_used, M), dtype=torch.float32, device=b.device)
+    assert out.shape == (T, n_used, M) and out.is_contiguous()
+    if path is None:
+        need = L.b200_mul_mat_id_workspace_bytes(t, M, K, n_used, T, nb1)
+        ws = torch.empty(need, dtype=torch.uint8, device=b.device)
+        _check(L.b200_mul_mat_id(t, w.data_ptr(), w.stride(1), w.stride(0), E, M, K, b.data_ptr(), nb1, ids.data_ptr(), ids.stride(0),
+                                 n_used, T, out.data_ptr(), ws.data_ptr(), need, _stream()), "b200_mul_mat_id")
+        return out
+    need = L.b200_mul_mat_id_path_workspace_bytes(t, M, K, E, n_used, T, nb1)
     ws = torch.empty(need, dtype=torch.uint8, device=b.device)
-    _check(L.b200_mul_mat_id(t, w.data_ptr(), w.stride(1), w.stride(0), E, M, K, b.data_ptr(), nb1, ids.data_ptr(), ids.stride(0),
-                             n_used, T, out.data_ptr(), ws.data_ptr(), need, _stream()), "b200_mul_mat_id")
-    return out
+    taken = C.c_int(0)
+    _check(L.b200_mul_mat_id_path(t, w.data_ptr(), w.stride(1), w.stride(0), E, M, K, b.data_ptr(), nb1, ids.data_ptr(), ids.stride(0),
+                                  n_used, T, out.data_ptr(), ws.data_ptr(), need, path, C.byref(taken), _stream()), "b200_mul_mat_id_path")
+    return out, taken.value
+
+
+def moe_route(ids: torch.Tensor, n_expert: int, nb1: int):
+    """The grouped GEMM's router alone (b200_moe_route): ids int32 [T, n_used] (any row stride) -> (tile_expert int32 [max_tiles],
+    col_src int32 [max_tiles, 128], col_dst int32 [max_tiles, 128])."""
+    T, n_used = ids.shape
+    assert ids.is_cuda and ids.dtype == torch.int32 and ids.stride(1) == 1
+    L = lib()
+    mt = int(L.b200_moe_route_max_tiles(n_expert, n_used, T))
+    te = torch.empty(mt, dtype=torch.int32, device=ids.device)
+    cs = torch.empty((mt, 128), dtype=torch.int32, device=ids.device)
+    cd = torch.empty((mt, 128), dtype=torch.int32, device=ids.device)
+    rc = L.b200_moe_route(ids.data_ptr(), ids.stride(0), n_expert, n_used, T, nb1, te.data_ptr(), cs.data_ptr(), cd.data_ptr(), _stream())
+    _check(0 if rc >= 0 else rc, "b200_moe_route")
+    assert rc == mt
+    return te, cs, cd
 
 
 class HostMulMat:

@@ -218,6 +218,10 @@ class Ref:
         b.ggml_nbytes.argtypes = [vp]
         b.ggml_flash_attn_ext.restype = vp
         b.ggml_flash_attn_ext.argtypes = [vp, vp, vp, vp, vp, C.c_float, C.c_float, C.c_float]
+        b.ggml_mul_mat_id.restype = vp
+        b.ggml_mul_mat_id.argtypes = [vp, vp, vp, vp]
+        b.ggml_view_2d.restype = vp
+        b.ggml_view_2d.argtypes = [vp, vp, i64, i64, C.c_size_t, C.c_size_t]
         b.ggml_rope_ext.restype = vp
         b.ggml_rope_ext.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int] + [C.c_float] * 6
         b.ggml_new_graph.restype = vp
@@ -229,19 +233,19 @@ class Ref:
         return b
 
     def _run_one_node(self, inputs, make_node, out_shape, mem: int):
-        """inputs: list of (ggml type, numpy array in ggml memory order, outermost first); make_node(ctx, tensors) -> node.
-        Returns the node's f32 data reshaped to out_shape."""
+        """inputs: list of (ggml type, numpy array in ggml memory order, outermost first[, ggml ne when the array's shape is not it,
+        e.g. quantised rows given as bytes]); make_node(ctx, tensors) -> node.  Returns the node's f32 data reshaped to out_shape."""
         b = self._graph_lib()
         ctx = b.ggml_init(_GgmlInitParams(mem + (64 << 20), None, False))
         assert ctx
         try:
             ts = []
-            for typ, arr in inputs:
+            for typ, arr, *given_ne in inputs:
                 if arr is None:
                     ts.append(None)
                     continue
                 arr = np.ascontiguousarray(arr)
-                ne = list(arr.shape[::-1]) + [1] * (4 - arr.ndim)
+                ne = list(given_ne[0]) + [1] * (4 - len(given_ne[0])) if given_ne else list(arr.shape[::-1]) + [1] * (4 - arr.ndim)
                 t = b.ggml_new_tensor_4d(ctx, typ, *ne)
                 assert b.ggml_nbytes(t) == arr.nbytes
                 C.memmove(b.ggml_get_data(t), arr.ctypes.data, arr.nbytes)
@@ -267,6 +271,23 @@ class Ref:
         mem = sum(a.nbytes for _, a in ins if a is not None) + B * N * H * DV * 4
         return self._run_one_node(ins, lambda ctx, t: self.base.ggml_flash_attn_ext(ctx, t[0], t[1], t[2], t[3], scale, 0.0, softcap),
                                   (B, N, H, DV), mem)
+
+    def mul_mat_id(self, t: int, w: np.ndarray, b: np.ndarray, ids: np.ndarray, n_expert_rows: int | None = None) -> np.ndarray:
+        """ggml_mul_mat_id on the CPU backend, with the ids built as llama builds them: a ggml_view_2d of the first n_used rows of an
+        i32 [n_expert_rows, T] tensor (the top-k argsort), so the view's row stride is n_expert_rows.  Layouts as Oracle.mul_mat_id:
+        w uint8 [E, M, row_bytes], b f32 [T, nb1, K], ids int32 [T, n_used]; returns f32 [T, n_used, M]."""
+        E, M, rb = w.shape
+        T, nb1, K = b.shape
+        n_used = ids.shape[1]
+        rows = n_expert_rows or E
+        full = np.zeros((T, rows), dtype=np.int32)          # the rows past n_used hold ids no view reads
+        full[:, :n_used] = ids
+        full[:, n_used:] = (np.arange(rows - n_used) % E)[None]
+        ins = [(t, np.ascontiguousarray(w, dtype=np.uint8), (K, M, E)), (GGML_TYPE_F32, np.ascontiguousarray(b, dtype=np.float32)), (26, full)]
+        mem = w.nbytes + b.nbytes + full.nbytes + T * n_used * M * 4 + (T * nb1 * K * 4 + (64 << 10))
+        bl = self._graph_lib()
+        return self._run_one_node(ins, lambda ctx, ts: bl.ggml_mul_mat_id(ctx, ts[0], ts[1], bl.ggml_view_2d(ctx, ts[2], n_used, T, rows * 4, 0)),
+                                  (T, n_used, M), mem)
 
     def rope_ext(self, x, pos, n_dims: int, mode: int, freq_base: float = 10000.0, freq_scale: float = 1.0, ext_factor: float = 0.0,
                  attn_factor: float = 1.0, beta_fast: float = 32.0, beta_slow: float = 1.0, n_ctx_orig: int = 0, freq_factors=None) -> np.ndarray:
@@ -405,3 +426,37 @@ def random_blocks(t: int, rows: int, k: int, rng: np.random.Generator, scale: fl
     elif t == Q6_K:
         put_half(208, u * scale / (64 * 32) * 2)
     return out.reshape(rows, nb * bb)
+
+
+def saturated_blocks(t: int, rows: int, k: int, rng: np.random.Generator) -> np.ndarray:
+    """K-quant rows whose integer fields are all at their extreme, so that one block's integer sum is as large as the format allows:
+    Q4_K / Q5_K every 6-bit scale and min 63 and every quant 15 / 31; Q6_K even rows scale -128 with q = 0 (sc (q - 32) = 4096),
+    odd rows scale 127 with q = 63 (3937).  With Q8_K activations of +-127 a block's main sum reaches 256 * 945 * 127 ~ 3.1e7 (Q4_K),
+    256 * 1953 * 127 ~ 6.3e7 (Q5_K) and 256 * 4096 * 127 ~ 1.3e8 (Q6_K), all above 2^24.  The fp16 super-scales are random."""
+    nb = k // BLOCK_ELEMS[t]
+    out = np.zeros((rows, nb, BLOCK_BYTES[t]), dtype=np.uint8)
+
+    def put_half(off, vals):
+        h = np.asarray(vals, dtype=np.float16).view(np.uint16)
+        out[:, :, off] = (h & 0xFF).astype(np.uint8)
+        out[:, :, off + 1] = (h >> 8).astype(np.uint8)
+
+    u = rng.uniform(0.5, 1.0, size=(rows, nb))
+    if t in (Q4_K, Q5_K):
+        out[:, :, 4:] = 0xFF                                  # scales / mins 63, (Q5_K: qh) and qs: every quant at its maximum
+        put_half(0, u * 2.0 ** -12)
+        put_half(2, rng.uniform(0.5, 1.0, size=(rows, nb)) * 2.0 ** -12)
+    elif t == Q6_K:
+        out[1::2, :, :192] = 0xFF                             # odd rows: q = 63 ...
+        out[1::2, :, 192:208] = 127                           # ... with scale 127
+        out[0::2, :, 192:208] = 0x80                          # even rows: q = 0 with scale -128
+        put_half(208, u * 2.0 ** -14)
+    else:
+        raise ValueError("saturated_blocks: K-quant types only")
+    return out.reshape(rows, nb * BLOCK_BYTES[t])
+
+
+def constant_sign_blocks(n: int, k: int, rng: np.random.Generator) -> np.ndarray:
+    """f32 [n, k] activations whose every 256-element block is one value of random sign and size: its Q8_K integers are all +-127."""
+    v = rng.uniform(0.25, 2.0, size=(n, k // 256)) * rng.choice([-1.0, 1.0], size=(n, k // 256))
+    return np.repeat(v, 256, axis=1).astype(np.float32)

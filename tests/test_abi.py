@@ -37,6 +37,13 @@ def test_every_attention_symbol_is_exported(lib):
         assert hasattr(lib, s), f"{s} declared in include/b200_attn.h but not exported by libb200qmm.so"
 
 
+def test_every_moe_symbol_is_exported(lib):
+    syms = declared_symbols("b200_moe.h")
+    assert syms == ["b200_moe_route", "b200_moe_route_max_tiles", "b200_mul_mat_id_path", "b200_mul_mat_id_path_workspace_bytes"]
+    for s in syms:
+        assert hasattr(lib, s), f"{s} declared in include/b200_moe.h but not exported by libb200qmm.so"
+
+
 def test_plugin_exports_every_symbol_its_header_declares():
     """libggml-b200.so (the drop-in boundary): the two dl entry points + the bench hooks of include/ggml-b200.h, and the
     kernel C ABI it embeds.  Symbol table only -- loading it needs libggml-base and calling it needs a GPU."""
@@ -51,7 +58,7 @@ def test_plugin_exports_every_symbol_its_header_declares():
     assert {"ggml_backend_init", "ggml_backend_score"} <= declared
     for s in sorted(declared):
         assert s in exported, f"{s} declared in include/ggml-b200.h but not exported by libggml-b200.so"
-    for s in declared_symbols("b200_qmm.h") + declared_symbols("b200_attn.h"):
+    for s in declared_symbols("b200_qmm.h") + declared_symbols("b200_attn.h") + declared_symbols("b200_moe.h"):
         assert s in exported, s
 
 
@@ -155,3 +162,37 @@ def test_attention_arguments_fail_before_touching_the_gpu(lib):
     assert lib.b200_attn_program(C.byref(a), None, None) == -1   # n_head not a multiple of n_head_kv
     assert b"n_head_kv" in lib.b200_qmm_last_error()
     assert lib.b200_attn_program(None, None, None) == -1
+
+
+def test_moe_arguments_fail_before_touching_the_gpu(lib):
+    """b200_mul_mat_id_path / b200_moe_route reject a bad path, nb1 or n_used on the host (no device memory is named)."""
+    lib.b200_qmm_last_error.restype = C.c_char_p
+    vp, i64 = C.c_void_p, C.c_int64
+    lib.b200_mul_mat_id_path.argtypes = [C.c_int, vp, i64, i64, i64, i64, i64, vp, i64, vp, i64, i64, i64, vp, vp, C.c_size_t, C.c_int,
+                                         C.POINTER(C.c_int), vp]
+    lib.b200_moe_route.restype = i64
+    lib.b200_moe_route.argtypes = [vp, i64, i64, i64, i64, i64, vp, vp, vp, vp]
+    lib.b200_moe_route_max_tiles.restype = i64
+    lib.b200_moe_route_max_tiles.argtypes = [i64, i64, i64]
+    taken = C.c_int(7)
+
+    def mmid(path, nb1=2, n_used=2, t=12, E=8, T=16, ws=1 << 30):
+        return lib.b200_mul_mat_id_path(t, None, 144, 144 * 64, E, 64, 256, None, nb1, None, E, n_used, T, None, None, ws, path,
+                                        C.byref(taken), None)
+
+    assert mmid(3) == -1 and b"path" in lib.b200_qmm_last_error()
+    assert taken.value == 0                                   # nothing ran
+    assert mmid(-1) == -1
+    assert mmid(0, nb1=3) == -1 and b"nb1" in lib.b200_qmm_last_error()
+    assert mmid(1, nb1=2, n_used=4) == -1
+    assert mmid(2, n_used=0, nb1=1) == -1 and b"n_used" in lib.b200_qmm_last_error()
+    assert mmid(1, n_used=-2, nb1=1) == -1
+    assert mmid(0, t=99) == -1                                # unknown type
+    assert mmid(2, ws=0) == -3                                # workspace too small
+    assert mmid(2, T=0) == 0                                  # no tokens: a no-op
+    assert lib.b200_moe_route_max_tiles(8, 2, 100) == 2 + 8   # ceil(200 / 128) + n_expert
+    assert lib.b200_moe_route_max_tiles(60, 4, 32) == 1 + 60
+    assert lib.b200_moe_route(C.c_void_p(16), 8, 8, 2, 4, 3, C.c_void_p(16), C.c_void_p(16), C.c_void_p(16), None) == -1   # nb1
+    assert lib.b200_moe_route(C.c_void_p(16), 8, 8, 0, 4, 1, C.c_void_p(16), C.c_void_p(16), C.c_void_p(16), None) == -1   # n_used
+    assert lib.b200_moe_route(C.c_void_p(16), 257, 257, 2, 4, 1, C.c_void_p(16), C.c_void_p(16), C.c_void_p(16), None) == -6
+    assert b"256" in lib.b200_qmm_last_error()

@@ -8,7 +8,7 @@ import os
 import numpy as np
 import pytest
 
-from oracle.oracle import ALL_TYPES, BLOCK_BYTES, BLOCK_ELEMS, Q8_K, TYPE_NAMES, act_type, random_blocks, row_bytes
+from oracle.oracle import ALL_TYPES, BLOCK_BYTES, BLOCK_ELEMS, Q4_K, Q5_K, Q6_K, Q8_K, TYPE_NAMES, act_type, random_blocks, row_bytes
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "qmm_golden.npz")
 
@@ -140,6 +140,33 @@ def test_mul_mat_id_routes_rows(oracle):
         for s in range(n_used):
             want = oracle.mul_mat(Q4_K, w[ids[tkn, s]], b[tkn])
             assert np.array_equal(out[tkn, s], want[0])
+
+
+@pytest.mark.parametrize("nb1_is_one", [True, False])
+@pytest.mark.parametrize("t", ALL_TYPES)
+def test_mul_mat_id_matches_ggml_cpu_mul_mat_id(oracle, ref, t, nb1_is_one):
+    """oracle.mul_mat_id against ggml_mul_mat_id on the reference's CPU backend, with the ids as llama builds them (the first n_used
+    rows of an [n_expert, T] tensor) and one token routed to the same expert twice.  Weights from the reference quantiser, O(1) outputs:
+    max-abs <= 1e-3, the bar of the reference-shaped mat-mul tests (the CPU backend quantises Q8_0 activations with its SIMD rounding,
+    the oracle with the _ref rounding; they differ at ties only).  K-quants share the Q8_K integers and differ in fp32 order only:
+    also <= 5e-6 sum_k |w_k x_k| per element."""
+    rng = np.random.default_rng(40 + t + 7 * nb1_is_one)
+    E, M, K, T, n_used = 4, 24, 4096, 6, 2
+    w = np.stack([ref.quantize_weights(t, (rng.standard_normal((M, K)) * 0.02).astype(np.float32)) for _ in range(E)])
+    nb1 = 1 if nb1_is_one else n_used
+    b = rng.standard_normal((T, nb1, K)).astype(np.float32)
+    ids = np.stack([rng.permutation(E)[:n_used] for _ in range(T)]).astype(np.int32)
+    ids[2] = [3, 3]                                           # the same expert in both slots of one token
+    want = ref.mul_mat_id(t, w, b, ids)
+    got = oracle.mul_mat_id(t, w, b, ids)
+    assert np.isfinite(want).all() and np.abs(want).max() > 0.5
+    assert np.abs(got - want).max() <= 1e-3, float(np.abs(got - want).max())
+    if t in (Q4_K, Q5_K, Q6_K):
+        deq = np.stack([np.stack([oracle.dequantize(t, w[e, m], K) for m in range(M)]) for e in range(E)])        # [E, M, K]
+        cols = b[np.arange(T)[:, None], np.arange(n_used)[None] % nb1]                                             # [T, n_used, K]
+        scale = np.einsum("tsk,tsmk->tsm", np.abs(cols), np.abs(deq[ids]))
+        assert (np.abs(got - want) <= 5e-6 * scale).all()
+    assert np.array_equal(got[2, 0], got[2, 1]) == (nb1 == 1)
 
 
 def test_empty_and_sizes(oracle):
