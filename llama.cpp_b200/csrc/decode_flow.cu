@@ -14,7 +14,9 @@
 //   * ONE weight stream per CTA for the whole token.  The producer warp walks the program ahead of the consumers and issues
 //     cp.async.bulk copies into a ring of 18 x 9.5 KB slots (full/empty mbarriers); weights do not depend on activations,
 //     so the stream crosses phase boundaries: while the consumers wait for a vector, the ring fills with the next phases'
-//     rows (25 MB on chip = ~4 us of HBM time, more than a dependency hop costs).
+//     rows (25 MB on chip = ~4 us of HBM time, more than a dependency hop costs).  The copies are evict-first in L2: the weights
+//     are read once per token, while the KV rows, the tagged vector slots and the inputs are read again; as normal-priority lines
+//     they now outlive the 4.6 GB stream instead of being pushed out by it (measured: DESIGN 5.3, 8).
 //   * Activations live in REGISTERS.  A lane is bound to one 256-weight k-block of the activation for a whole phase
 //     (K = 4096: lane l <-> block l % 16, two rows per warp step; K = 14336: two warps per row, 28 lanes each), so the
 //     quantised activation block (64 words) is loaded once per phase and a block dot product reads only its 144..210
@@ -425,6 +427,7 @@ __device__ __forceinline__ void producer_loop(const FlowPhase * __restrict__ ph,
     uint32_t * pdesc = reinterpret_cast<uint32_t *>(smem + OFF_DESC + 2 * 384);
     const int cta = (int)blockIdx.x, grid = (int)gridDim.x;
     unsigned g = 0;                                                  // pieces issued so far (this CTA, whole program)
+    const uint64_t l2_pol = l2_evict_first_policy();                 // evict-first weight stream: see the header
     int pi = next_matvec(ph, 0, n_phases), buf = 0;
     if (pi < n_phases) {
         const uint32_t * src = reinterpret_cast<const uint32_t *>(ph + pi);
@@ -494,7 +497,7 @@ __device__ __forceinline__ void producer_loop(const FlowPhase * __restrict__ ph,
                     }
                     if (lane == 0) mbar_expect_tx(full + slot, tx);
                     __syncwarp();
-                    if (cnt) bulk_g2s(dst, src, cnt, full + slot);
+                    if (cnt) bulk_g2s_hint(dst, src, cnt, full + slot, l2_pol);
                     g++;
                 }
             }
@@ -529,6 +532,7 @@ __device__ __forceinline__ void producer_loop(const FlowPhase * __restrict__ ph,
     uint32_t * pdesc = reinterpret_cast<uint32_t *>(smem + OFF_DESC + 2 * 384);
     const int cta = (int)blockIdx.x, grid = (int)gridDim.x;
     unsigned gbase = 0;                                              // pieces of the phases before the current one (this CTA)
+    const uint64_t l2_pol = l2_evict_first_policy();                 // evict-first weight stream: see the header
     int pi = next_matvec(ph, 0, n_phases), buf = 0;
     if (pi < n_phases) {
         const uint32_t * src = reinterpret_cast<const uint32_t *>(ph + pi);
@@ -575,8 +579,8 @@ __device__ __forceinline__ void producer_loop(const FlowPhase * __restrict__ ph,
                     const uint32_t off0 = (uint32_t)(reinterpret_cast<uintptr_t>(g0) & 15), off1 = (uint32_t)(reinterpret_cast<uintptr_t>(g1) & 15);
                     const uint32_t c0 = (off0 + total + 15u) & ~15u, c1 = sub == 2 ? ((off1 + total + 15u) & ~15u) : 0u;
                     mbar_expect_tx(full + slot, c0 + c1);
-                    bulk_g2s(sl, g0 - off0, c0, full + slot);
-                    if (sub == 2) bulk_g2s(sl + sub_pitch(R, row_bytes), g1 - off1, c1, full + slot);
+                    bulk_g2s_hint(sl, g0 - off0, c0, full + slot, l2_pol);
+                    if (sub == 2) bulk_g2s_hint(sl + sub_pitch(R, row_bytes), g1 - off1, c1, full + slot, l2_pol);
                 } else {
                     // one copy per (sub-piece, row): this segment's blocks of the row
                     const int rpitch = row_pitch(seg, bb);
@@ -593,7 +597,7 @@ __device__ __forceinline__ void producer_loop(const FlowPhase * __restrict__ ph,
                         for (int r = 0; r < nr; r++) {
                             const uint8_t * gp = (j ? w1 : w0) + (int64_t)(r0 + r) * (j ? rs1 : rs0) + koff;
                             const uint32_t off = (uint32_t)(reinterpret_cast<uintptr_t>(gp) & 15);
-                            bulk_g2s(sl + (j * R + r) * rpitch, gp - off, (off + total + 15u) & ~15u, full + slot);
+                            bulk_g2s_hint(sl + (j * R + r) * rpitch, gp - off, (off + total + 15u) & ~15u, full + slot, l2_pol);
                         }
                 }
             }

@@ -1,4 +1,4 @@
-// gemv_blockdot.cuh -- pieces shared by the decode GEMV kernels (gemv2.cu, gemv3.cu): tile configuration, the
+// gemv_blockdot.cuh -- pieces shared by the decode GEMV kernels (gemv2.cu, gemv3.cu, decode_flow.cu): tile configuration, the
 // mbarrier / cp.async.bulk PTX wrappers and the per-lane 256-weight block dot products.
 #pragma once
 #include "qmm_formats.cuh"
@@ -40,6 +40,17 @@ __device__ __forceinline__ void mbar_wait(uint64_t * bar, uint32_t parity) {
 __device__ __forceinline__ void bulk_g2s(void * smem_dst, const void * gsrc, uint32_t bytes, uint64_t * bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n"
                  ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+}
+// An L2 policy that marks every line it covers evict-first, and bulk_g2s under such a policy: data read once on its way to shared memory
+// then leaves L2 before the lines that are read again.
+__device__ __forceinline__ uint64_t l2_evict_first_policy() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;\n" : "=l"(pol));
+    return pol;
+}
+__device__ __forceinline__ void bulk_g2s_hint(void * smem_dst, const void * gsrc, uint32_t bytes, uint64_t * bar, uint64_t policy) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;\n"
+                 ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)), "l"(policy) : "memory");
 }
 __device__ __forceinline__ int dp4a_us(uint32_t a_unsigned, uint32_t b_signed, int c) {
     int d;

@@ -5,10 +5,21 @@ Per phase and CTA the kernel stamps the globaltimer at: 0 phase entered, 1 input
 the dependency it sits on: from the moment the LAST producer CTA of the previous phase finished (max of stamp 3 of the previous
 phase) to the moment the last CTA of this phase finished.  CTAs without rows in a phase leave no stamps 1..3."""
 import collections
+import json
+import os
 import struct
 import sys
 
 import numpy as np
+
+
+def hbm_peak() -> float:
+    """GB/s: the measured peak when MEASURED_PEAKS.json exists, else the H100 SXM data sheet's 3.35 TB/s (as bench.py)"""
+    p = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")
+    if os.path.exists(p):
+        return float(json.load(open(p))["hbm_gbs"])
+    return 3350.0
+
 
 raw = open(sys.argv[1], "rb").read()
 n, grid = struct.unpack("ii", raw[:8])
@@ -19,7 +30,7 @@ t = body.reshape(-1, TN, 160)[:n, :, :grid].astype(np.float64)
 FINE = TN >= 11 and (t[:, 8] > 0).any()
 KN = {0: "MATVEC", 1: "ATTN", 2: "COPY", 3: "ADD"}
 BB = {12: 144, 13: 176, 14: 210}
-PEAK = 6486.8  # GB/s, MEASURED_PEAKS.json
+PEAK = hbm_peak()
 
 
 def bytes_of(r):
@@ -73,7 +84,7 @@ for i in range(n):
         f[5] += (t[i, 10][h10].max() - end_prev) if h10.any() else 0.0        # last warp of the last CTA done
     total_span += span
     end_prev = end
-print(f"{n} phases, grid {grid}; token span {(ts[ts > 0].max() - t0) / 1e3:.1f} us; sum of phase spans {total_span / 1e3:.1f} us")
+print(f"{n} phases, grid {grid}; token span {(ts[ts > 0].max() - t0) / 1e3:.1f} us; sum of phase spans {total_span / 1e3:.1f} us; ideal = weight bytes / {PEAK:.0f} GB/s")
 print(f"{'phase (kind, K, sum M, type)':42s} {'n':>4s} {'span us':>8s} {'ideal us':>8s} {'x-arrive':>8s} {'quantise':>8s} {'stream':>8s} {'skew':>6s} {'w0 wait kcyc':>12s} {'w0 comp kcyc':>12s}")
 for key, (c, span, arr, qd, strm, skew, tw, tc) in agg.items():
     ideal = bytes_of((0 if key[0] == "MATVEC" else 1, key[1], key[2], key[3])) / PEAK / 1e3
