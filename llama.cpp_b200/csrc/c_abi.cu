@@ -1,4 +1,4 @@
-// c_abi.cu -- the extern "C" surface declared in include/b200_qmm.h, include/b200_attn.h and include/b200_moe.h.  Thin: argument checks, workspace carving,
+// c_abi.cu -- the extern "C" surface declared in include/b200_qmm.h, include/b200_attn.h, include/b200_moe.h and include/b200_flow.h.  Thin: argument checks, workspace carving,
 // regime selection (decode GEMV vs prefill GEMM), error text.  No compute happens on the host and there is no CPU
 // fallback: if CUDA is unusable every compute entry point fails loudly.
 #include <atomic>
@@ -9,6 +9,7 @@
 #include "../../include/b200_qmm.h"
 #include "../../include/b200_attn.h"
 #include "../../include/b200_moe.h"
+#include "../../include/b200_flow.h"
 #include "qmm_formats.cuh"
 #include <vector>
 #include <string.h>
@@ -21,6 +22,10 @@
 namespace qmm {
 static std::atomic<uint64_t> g_launches{0};
 void note_launch(int n) { g_launches.fetch_add((uint64_t)n, std::memory_order_relaxed); }
+// decode_flow.cu: the Q8_K hand-over as the recorded phases carry it (b200_flow_q8k_plan, b200_flow_q8k_reuse)
+int    flow_q8k_block_of(const FlowMatvec & p, int cta);          // the block CTA `cta` quantises, -1: none (or the phase emits no Q8_K blocks)
+size_t flow_q8k_words(const FlowMatvec & p);                      // tagged words of the phase's Q8_K blocks (out[1].ll), 0: none
+bool   flow_reads_q8k(const FlowMatvec & p);                      // the phase's input is a Q8_K vector
 static bool g_pdl = false;
 void set_pdl(bool on) { g_pdl = on; }
 bool pdl_enabled() { return g_pdl; }
@@ -346,6 +351,81 @@ int b200_flow_selftest_postponed_rope(void) {
     if (at.v.ll == qv.ll || at.v.ll != fb.phases()[1].mv.out[0].ll) return 7;   // v: the slots of the second phase's first matrix
     if (at.k.ll != fb.phases()[1].mv.out[1].ll) return 8;
     return 0;
+}
+
+int b200_flow_q8k_plan(int producer_mode, int64_t M, int64_t K_in, int consumer_norm, int grid, int * block_of_cta) {
+    if ((producer_mode != 0 && producer_mode != 2) || M <= 0 || M > FLOW_MAX_K || K_in <= 0 || K_in > FLOW_MAX_K || grid <= 0 || grid > 4096 || !block_of_cta)
+        return fail(B200_E_INVALID, "b200_flow_q8k_plan: bad arguments");
+    const uintptr_t fake = 0x100000;                           // aligned, never dereferenced on the host
+    FlowBuilder fb;
+    fb.reset(reinterpret_cast<uint64_t *>(fake * 64), 1 << 20, grid);
+    FlowBuilder::MatvecDesc up;
+    up.nmat = producer_mode == 2 ? 2 : 1; up.K = (int)K_in; up.mode = producer_mode; up.x = (const float *)(fake * 1);
+    up.norm_w = (const float *)(fake * 2); up.eps = 1e-5f; up.dst[0] = (float *)(fake * 3);
+    for (int j = 0; j < up.nmat; j++) { up.w[j] = (const uint8_t *)(fake * (8 + j)); up.row_stride[j] = K_in / 256 * 144; up.M[j] = (int)M; up.type[j] = T_Q4_K; }
+    FlowBuilder::MatvecDesc down;
+    down.nmat = 1; down.K = (int)M; down.mode = 0; down.x = up.dst[0]; down.norm_w = consumer_norm ? (const float *)(fake * 4) : nullptr; down.eps = 1e-5f;
+    down.w[0] = (const uint8_t *)(fake * 10); down.row_stride[0] = M / 256 * 144; down.M[0] = 4096; down.type[0] = T_Q4_K; down.dst[0] = (float *)(fake * 5);
+    if (!fb.add_matvec(up) || !fb.add_matvec(down)) return fail(B200_E_UNSUPPORTED, "b200_flow_q8k_plan: phase not representable");
+    const bool q8k = flow_reads_q8k(fb.phases()[1].mv);
+    for (int c = 0; c < grid; c++) block_of_cta[c] = flow_q8k_block_of(fb.phases()[0].mv, c);
+    return q8k ? 1 : 0;
+}
+
+int b200_flow_q8k_reuse(int n_layers, int64_t n_ff, int64_t pool_elems, int grid, int * n_q8k, int * min_phases) {
+    if (n_layers <= 0 || n_layers > 256 || n_ff <= 0 || n_ff > FLOW_MAX_K || pool_elems <= 0 || grid < 32 || grid > 4096 || !n_q8k || !min_phases)
+        return fail(B200_E_INVALID, "b200_flow_q8k_reuse: bad arguments");
+    const uintptr_t fake = 0x100000;                           // aligned, never dereferenced on the host
+    uint64_t * const pool = reinterpret_cast<uint64_t *>(fake * 4096);
+    FlowBuilder fb;
+    fb.reset(pool, (size_t)pool_elems, grid);
+    const int E = 4096, D = 128, H = 32, HKV = 8;
+    auto vecp = [&](int l, int j) { return (float *)(fake * (16 + 16 * (size_t)l + j)); };
+    auto mv = [&](int nmat, int K, int mode, const float * x, const float * norm_w, const float * resid, const int * M, float * d0, float * d1, float * d2) {
+        FlowBuilder::MatvecDesc d;
+        d.nmat = nmat; d.K = K; d.mode = mode; d.x = x; d.norm_w = norm_w; d.residual = resid; d.eps = 1e-5f;
+        float * dst[3] = {d0, d1, d2};
+        for (int j = 0; j < nmat; j++) { d.w[j] = (const uint8_t *)(fake * 8); d.row_stride[j] = K / 256 * 144; d.M[j] = M[j]; d.type[j] = T_Q4_K; d.dst[j] = dst[j]; }
+        return fb.add_matvec(d);
+    };
+    const float * h = (const float *)(fake * 1), * nw = (const float *)(fake * 2);
+    for (int l = 0; l < n_layers; l++) {
+        const int mqkv[3] = {H * D, HKV * D, HKV * D}, me[1] = {E}, mff[2] = {(int)n_ff, (int)n_ff};
+        FlowAttn a;
+        memset(&a, 0, sizeof(a));
+        a.n_head = H; a.n_head_kv = HKV; a.head_dim = D; a.n_dims = D; a.rope_mode = 0; a.n_kv = 256;
+        a.kview = (const void *)(fake * 11); a.vview = (const void *)(fake * 12); a.k_nb1 = 2048; a.k_nb2 = 256; a.v_nb1 = 2048; a.v_nb2 = 256;
+        if (!mv(3, E, 0, h, nw, nullptr, mqkv, vecp(l, 0), vecp(l, 1), vecp(l, 2)) || !fb.add_attn(a, vecp(l, 0), vecp(l, 1), vecp(l, 2), vecp(l, 3)) ||
+            !mv(1, E, 1, vecp(l, 3), nullptr, h, me, vecp(l, 4), nullptr, nullptr) || !mv(2, E, 2, vecp(l, 4), nw, nullptr, mff, vecp(l, 5), nullptr, nullptr) ||
+            !mv(1, (int)n_ff, 1, vecp(l, 5), nullptr, vecp(l, 4), me, vecp(l, 6), nullptr, nullptr))
+            return fail(B200_E_UNSUPPORTED, "b200_flow_q8k_reuse: phase not representable");
+        h = vecp(l, 6);
+    }
+    // the slot ranges every phase writes, then the fewest phases between two writes of one slot
+    struct Range { size_t lo, hi; int phase; };
+    std::vector<Range> rs;
+    const auto & ph = fb.phases();
+    int nq = 0;
+    auto add = [&](const uint64_t * ll, size_t n, int i) { if (ll && n) rs.push_back(Range{(size_t)(ll - pool), (size_t)(ll - pool) + n, i}); };
+    for (int i = 0; i < (int)ph.size(); i++) {
+        if (ph[i].kind == FLOW_MATVEC) {
+            const FlowMatvec & m = ph[i].mv;
+            for (int j = 0; j < (m.mode == 2 ? 1 : m.nmat); j++) add(m.out[j].ll, (size_t)m.M[j], i);
+            add(m.out[1].ll, flow_q8k_words(m), i);
+            nq += flow_reads_q8k(m) ? 1 : 0;
+        } else if (ph[i].kind == FLOW_ATTN) {
+            const FlowAttn & at = ph[i].at;
+            add(at.out.ll, (size_t)at.n_head * at.head_dim, i);
+            add(at.part_ll, (size_t)at.n_head * at.nsplit * (at.head_dim + 2), i);
+        }
+    }
+    int dist = (int)ph.size();
+    for (size_t x = 0; x < rs.size(); x++)
+        for (size_t y = x + 1; y < rs.size(); y++)
+            if (rs[x].lo < rs[y].hi && rs[y].lo < rs[x].hi && rs[x].phase != rs[y].phase) dist = std::min(dist, std::abs(rs[y].phase - rs[x].phase));
+    *n_q8k = nq;
+    *min_phases = dist;
+    return B200_OK;
 }
 
 size_t b200_mul_mat_id_workspace_bytes(int type, int64_t M, int64_t K, int64_t n_used, int64_t T, int64_t nb1) {

@@ -32,6 +32,11 @@
 // Slot reuse: the pool of tagged slots is carved round-robin by the host (FlowBuilder).  Every mat-vec phase validates ALL of
 // its input vector before it produces anything, so by the time any CTA produces the output of phase p + 2, every consumer of
 // phase p's input has finished reading it; the pool holds several layers' worth of outputs, far more than that distance.
+// The Q8_K hand-over (q8k_block_of) keeps this.  A SwiGLU phase p that emits Q8_K blocks also writes its f32 slots; those are read by
+// the CTAs of phase p that quantise them, which are producers of p and read them before they leave p, and by any other reader as
+// before.  The Q8_K words are written in phase p and read by the consumer phase, which validates all of them before it produces
+// anything.  So neither is read later than any other vector of phase p, and with the Q8_K regions carved from the same pool it still
+// holds many layers between two writes of a slot (tests/test_flow_q8k.py measures that distance for Llama-3-8B).
 //
 // All spin loops are bounded and __trap(): a lost producer must fail the launch, never hang the GPU.
 #include <cuda_fp16.h>
@@ -67,6 +72,15 @@ constexpr int FL_MAXBLK = FLOW_MAX_K / 256;                // 64
 constexpr int FL_PU = 5;                                   // activation blocks per warp and prologue pass
 static_assert(FL_PU * FL_NW * 256 >= FLOW_MAX_NORM_K, "a fused RMS_NORM must fit one prologue pass");
 constexpr int ACT_PITCH = 272;                             // bytes per quantised block in shared memory (skewed)
+// A SwiGLU output handed to the next mat-vec as Q8_K blocks (see "Q8_K hand-over" below).  These are not in decode_flow.cuh: the
+// plugin's C++ objects compile against that header, and a checkout without the reference sources links prebuilt objects only while
+// it is unchanged.
+constexpr uint32_t FLOW_VEC_Q8K = 2;                       // FlowVec::flags: ll holds Q8_K blocks of FL_Q8K_WORDS tagged words, not f32 values
+constexpr int FLOW_MV_Q8K_OUT = 1;                         // FlowMatvec::plan_pad_[0]: the SwiGLU phase also writes out[0] as Q8_K blocks to out[1].ll
+constexpr int FL_Q8K_WORDS = 73;                           // tagged words per block: 64 of 4 int8, 8 of 2 int16 sums of 16, d (f32 bits).  A vector
+                                                           // of n blocks holds all int8 words first (block-major), then the sums, then the scales:
+                                                           // word i of each part is what the prologue keeps at byte 4 i of ACT_*
+constexpr int FL_Q8K_PAIRS = (FL_Q8K_WORDS * FL_MAXBLK / 2 + FL_CTHREADS - 1) / FL_CTHREADS;   // 16-byte loads per consumer thread (11)
 constexpr int FL_TK = 4 * FL_CTHREADS;                     // keys per attention tile
 constexpr int FL_KG = FL_CTHREADS / 16;                    // key groups in the P.V pass
 
@@ -103,10 +117,11 @@ __device__ __forceinline__ uint64_t ld_slot(const uint64_t * p) {
 __device__ __forceinline__ void ld_slot2(const uint64_t * p, uint64_t & a, uint64_t & b) {
     asm volatile("ld.relaxed.gpu.global.v2.u64 {%0, %1}, [%2];\n" : "=l"(a), "=l"(b) : "l"(p) : "memory");
 }
-__device__ __forceinline__ void st_slot(uint64_t * p, uint32_t tag, float v) {
-    const uint64_t w = ((uint64_t)tag << 32) | (uint64_t)__float_as_uint(v);
+__device__ __forceinline__ void st_word(uint64_t * p, uint32_t tag, uint32_t v) {
+    const uint64_t w = ((uint64_t)tag << 32) | (uint64_t)v;
     asm volatile("st.relaxed.gpu.global.u64 [%0], %1;\n" ::"l"(p), "l"(w) : "memory");
 }
+__device__ __forceinline__ void st_slot(uint64_t * p, uint32_t tag, float v) { st_word(p, tag, __float_as_uint(v)); }
 // Bounded waits: a lost producer (or a missing bulk copy) must fail the launch, never hang the GPU.  Wall-clock bound (globaltimer,
 // checked every 256 polls): 4 s is ~3 orders of magnitude above a whole token.
 __device__ __forceinline__ unsigned long long gtime() {
@@ -393,7 +408,19 @@ template <> struct RegDot<T_Q6_K> {
 
 // ------------------------------------------------------------------------------------------------ geometry shared by producer and consumers
 // first row of CTA `cta` of matrix m: the host planned rq = M / grid rows per CTA and gives the first rr = M % grid CTAs one more
-__device__ __forceinline__ int row_begin(const FlowMatvec & p, int m, int cta) { const int r = p.rr[m]; return cta * p.rq[m] + (cta < r ? cta : r); }
+__host__ __device__ __forceinline__ int row_begin(const FlowMatvec & p, int m, int cta) { const int r = p.rr[m]; return cta * p.rq[m] + (cta < r ? cta : r); }
+
+// Q8_K hand-over.  A mat-vec without a fused RMS_NORM quantises each 256-block of its input from those 256 values alone, so when the
+// input is a SwiGLU output the block can be quantised once, in the phase that produces it, and every consumer CTA reads the same bytes
+// (FL_Q8K_WORDS tagged words per block instead of 256 f32 slots, and no quantisation in the consumers' prologue).  Block b is quantised
+// by the CTA that owns its last row, 256 b + 255: after its own rows it polls the block's f32 slots and one warp writes the words.  Rows
+// are contiguous per CTA, so a CTA that owns at most 256 rows owns at most one such row; the host takes this route only when every
+// block gets exactly one quantiser (FlowBuilder::add_matvec).  Returns the block `cta` quantises, -1 for none.
+__host__ __device__ __forceinline__ int q8k_block_of(const FlowMatvec & p, int cta) {
+    const int rb = row_begin(p, 0, cta), re = row_begin(p, 0, cta + 1);
+    const int b = (re >> 8) - 1;                                       // the last block whose last row lies below re
+    return b >= 0 && 256 * b + 255 >= rb ? b : -1;
+}
 
 struct PieceGeom {
     int nblk, contiguous[3], row_bytes[3], sub;
@@ -618,8 +645,8 @@ __device__ __forceinline__ void producer_loop(const FlowPhase * __restrict__ ph,
 
 // ------------------------------------------------------------------------------------------------ Q8_K quantisation of one 256-block held by a warp
 // quantize_row_q8_K_ref (ggml-quants.c:2768-2805): lane l holds elements 8l..8l+7; the FIRST element of largest magnitude decides
-// scale and sign.  Writes the int8 values (skewed pitch), the 16 sums of 16 and the scale to shared memory.
-__device__ __forceinline__ void quant_block(const float (&v)[8], int b, int lane, uint8_t * act) {
+// scale and sign.  Gives the lane its 8 int8 values (packed), the sum of its group of 16 (both lanes of the group hold it) and the scale.
+__device__ __forceinline__ void quant_lane(const float (&v)[8], uint2 & packed, int & s16, float & d) {
     unsigned mloc = 0;
 #pragma unroll
     for (int i = 0; i < 8; i++) { const unsigned a = (v[i] == v[i]) ? (__float_as_uint(v[i]) & 0x7fffffffu) : 0u; mloc = a > mloc ? a : mloc; }
@@ -632,7 +659,7 @@ __device__ __forceinline__ void quant_block(const float (&v)[8], int b, int lane
     const float maxv = __shfl_sync(0xffffffffu, mine, wl);
     const float amax = __uint_as_float(mall);
     int q[8];
-    float d = 0.0f;
+    d = 0.0f;
     if (amax > 0.0f) {
         const float iscale = __fdiv_rn(-127.0f, maxv);
 #pragma unroll
@@ -642,14 +669,32 @@ __device__ __forceinline__ void quant_block(const float (&v)[8], int b, int lane
 #pragma unroll
         for (int i = 0; i < 8; i++) q[i] = 0;
     }
-    uint2 packed;
     packed.x = (uint32_t)(q[0] & 0xFF) | ((uint32_t)(q[1] & 0xFF) << 8) | ((uint32_t)(q[2] & 0xFF) << 16) | ((uint32_t)(q[3] & 0xFF) << 24);
     packed.y = (uint32_t)(q[4] & 0xFF) | ((uint32_t)(q[5] & 0xFF) << 8) | ((uint32_t)(q[6] & 0xFF) << 16) | ((uint32_t)(q[7] & 0xFF) << 24);
-    *reinterpret_cast<uint2 *>(act + (size_t)b * ACT_PITCH + 8 * lane) = packed;
     const int s8 = q[0] + q[1] + q[2] + q[3] + q[4] + q[5] + q[6] + q[7];
-    const int s16 = s8 + __shfl_xor_sync(0xffffffffu, s8, 1);
+    s16 = s8 + __shfl_xor_sync(0xffffffffu, s8, 1);
+}
+// ... written to the prologue's shared-memory layout: the int8 values (skewed pitch), the 16 sums of 16 and the scale of block b
+__device__ __forceinline__ void quant_block(const float (&v)[8], int b, int lane, uint8_t * act) {
+    uint2 packed;
+    int s16;
+    float d;
+    quant_lane(v, packed, s16, d);
+    *reinterpret_cast<uint2 *>(act + (size_t)b * ACT_PITCH + 8 * lane) = packed;
     if ((lane & 1) == 0) reinterpret_cast<int16_t *>(act + ACT_BS + (size_t)b * 32)[lane >> 1] = (int16_t)s16;
     if (lane == 0) reinterpret_cast<float *>(act + ACT_D)[b] = d;
+}
+// ... written as block b of a Q8_K vector of nblk blocks (tagged words, see FL_Q8K_WORDS)
+__device__ __forceinline__ void quant_block_ll(const float (&v)[8], int b, int nblk, int lane, uint64_t * ll, uint32_t tag) {
+    uint2 packed;
+    int s16;
+    float d;
+    quant_lane(v, packed, s16, d);
+    st_word(ll + 64 * b + 2 * lane, tag, packed.x);
+    st_word(ll + 64 * b + 2 * lane + 1, tag, packed.y);
+    const int s16_next = __shfl_down_sync(0xffffffffu, s16, 2);      // the next group's sum: two groups per word
+    if ((lane & 3) == 0) st_word(ll + 64 * nblk + 8 * b + (lane >> 2), tag, ((uint32_t)s16 & 0xFFFFu) | ((uint32_t)s16_next << 16));
+    if (lane == 0) st_word(ll + 72 * nblk + b, tag, __float_as_uint(d));
 }
 
 // (FLOW_AB_BATCH_QUANT builds only: measured 420 vs 426 tok/s for the serial form, lease X -- the extra live registers cost more than the
@@ -701,6 +746,53 @@ __device__ __forceinline__ void quant_blocks(const float (&v)[NU][8], const int 
             *reinterpret_cast<uint2 *>(act + (size_t)b[u] * ACT_PITCH + 8 * lane) = packed;
             if ((lane & 1) == 0) reinterpret_cast<int16_t *>(act + ACT_BS + (size_t)b[u] * 32)[lane >> 1] = (int16_t)s16;
             if (lane == 0) reinterpret_cast<float *>(act + ACT_D)[b[u]] = d[u];
+        }
+    }
+}
+
+// The prologue of a mat-vec whose input is a Q8_K vector: every consumer thread issues all of its 16-byte loads of the blocks' words at
+// once, spins on the first until it is valid, then re-polls whatever is still stale as a batch (the rule of vec_ld8_finish_blocks), and
+// stores the payload where quant_block would have put it.  (An odd word count leaves one word at the end that nobody writes.)
+__device__ __forceinline__ void q8k_load(const FlowVec & x, int nblk, EpochT epoch, int tid, uint8_t * act) {
+    const int nw = FL_Q8K_WORDS * nblk, npair = (nw + 1) >> 1;
+    const uint32_t want = want_tag(x, epoch);
+    uint64_t r[FL_Q8K_PAIRS][2];
+#pragma unroll
+    for (int u = 0; u < FL_Q8K_PAIRS; u++) {
+        const int j = tid + u * FL_CTHREADS;
+        r[u][0] = r[u][1] = (uint64_t)want << 32;                     // (pairs past the end count as valid)
+        if (j < npair) ld_slot2(x.ll + 2 * j, r[u][0], r[u][1]);
+        if (2 * j + 1 >= nw) r[u][1] = (uint64_t)want << 32;
+    }
+    long long spins = 0;
+    while ((uint32_t)(r[0][0] >> 32) != want || (uint32_t)(r[0][1] >> 32) != want) {
+        spin_fail(spins);
+        ld_slot2(x.ll + 2 * tid, r[0][0], r[0][1]);
+        if (2 * tid + 1 >= nw) r[0][1] = (uint64_t)want << 32;
+    }
+    for (;;) {
+        bool stale = false;
+#pragma unroll
+        for (int u = 1; u < FL_Q8K_PAIRS; u++) {
+            if ((uint32_t)(r[u][0] >> 32) != want || (uint32_t)(r[u][1] >> 32) != want) {
+                const int j = tid + u * FL_CTHREADS;
+                ld_slot2(x.ll + 2 * j, r[u][0], r[u][1]);
+                if (2 * j + 1 >= nw) r[u][1] = (uint64_t)want << 32;
+                stale = true;
+            }
+        }
+        if (!stale) break;
+        spin_fail(spins);
+    }
+#pragma unroll
+    for (int u = 0; u < FL_Q8K_PAIRS; u++) {
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+            const int s = 2 * (tid + u * FL_CTHREADS) + h;
+            if (s < nw) {
+                const int off = s < 64 * nblk ? (s >> 6) * ACT_PITCH + 4 * (s & 63) : (s < 72 * nblk ? ACT_BS : ACT_D - 32 * nblk) + 4 * (s - 64 * nblk);
+                *reinterpret_cast<uint32_t *>(act + off) = (uint32_t)r[u][h];
+            }
         }
     }
 }
@@ -858,9 +950,13 @@ __device__ __forceinline__ void matvec_phase(const FlowMatvec & p, int pi, Ctx &
 
     // ---- activation prologue: warp w owns blocks w, w + 8, ...; lane l owns elements 8l..8l+7 of a block.  Passes of 35 blocks
     //      (5 per warp); a fused RMS_NORM needs the whole vector before anything is quantised, so it is limited to one pass
-    //      (K <= FLOW_MAX_NORM_K = 8192 = 32 blocks).
-    const bool norm = p.norm_w != nullptr;
-    for (int base = 0; base < nblk; base += FL_PU * FL_NW) {
+    //      (K <= FLOW_MAX_NORM_K = 8192 = 32 blocks).  A Q8_K input (no norm, no hidden state to keep) is only copied in.
+    const bool norm = p.norm_w != nullptr, q8k = (p.x.flags & FLOW_VEC_Q8K) != 0;
+    if (q8k) {
+        q8k_load(p.x, nblk, epoch, tid, act);
+        stamp(c, pi, 1);
+    }
+    for (int base = 0; !q8k && base < nblk; base += FL_PU * FL_NW) {
         float xv[FL_PU][8];
         uint64_t raw[FL_PU][8];
 #pragma unroll
@@ -1076,6 +1172,18 @@ __device__ __forceinline__ void matvec_phase(const FlowMatvec & p, int pi, Ctx &
         const int rb = row_begin(p, 0, cta), re = row_begin(p, 0, cta + 1);
         mc.out = p.out[0];
         for (int t = tid; t < re - rb; t += FL_CTHREADS) mv_epilogue(mc, rb + t, __fadd_rn(part[t], part[FLOW_PART_ROWS + t]), 0.0f);
+    }
+    if ((p.plan_pad_[0] & FLOW_MV_Q8K_OUT) && warp == 0) {             // Q8_K hand-over: this CTA's block, once its rows are written
+        const int b = q8k_block_of(p, cta);
+        if (b >= 0) {
+            FlowVec y;                                                   // the phase's own f32 output (a producer of it may read it)
+            y.plain = nullptr; y.ll = p.out[0].ll; y.tag = (uint32_t)pi + 1u; y.flags = 0;
+            uint64_t raw[8];
+            float v[8];
+            vec_ld8_issue(y, 256 * b + 8 * lane, raw);
+            vec_ld8_finish(y, 256 * b + 8 * lane, epoch, raw, v);
+            quant_block_ll(v, b, p.M[0] >> 8, lane, p.out[1].ll, tag);
+        }
     }
     stamp(c, pi, 3);
 }
@@ -1565,6 +1673,22 @@ FlowOut FlowBuilder::out(float * p, int n, bool want_ll) {
 
 static int flow_block_bytes(int t) { return t == T_Q4_K ? 144 : (t == T_Q5_K ? 176 : (t == T_Q6_K ? 210 : 0)); }
 
+// every 256-block of the phase's output has exactly one quantiser (false when some CTA owns more than 256 rows)
+static bool q8k_one_quantiser_per_block(const FlowMatvec & p, int grid) {
+    std::vector<int> n((size_t)(p.M[0] / 256), 0);
+    for (int c = 0; c < grid; c++) {
+        const int b = q8k_block_of(p, c);
+        if (b >= 0) n[(size_t)b]++;
+    }
+    for (int k : n) if (k != 1) return false;
+    return true;
+}
+
+// host-side views of the Q8_K hand-over for the plan checks of the C ABI (c_abi.cu)
+int    flow_q8k_block_of(const FlowMatvec & p, int cta) { return (p.plan_pad_[0] & FLOW_MV_Q8K_OUT) ? q8k_block_of(p, cta) : -1; }
+size_t flow_q8k_words(const FlowMatvec & p) { return (p.plan_pad_[0] & FLOW_MV_Q8K_OUT) ? (size_t)FL_Q8K_WORDS * (p.M[0] / 256) : 0; }
+bool   flow_reads_q8k(const FlowMatvec & p) { return (p.x.flags & FLOW_VEC_Q8K) != 0; }
+
 bool FlowBuilder::matvec_ok(const MatvecDesc & d) const {
     if (d.nmat < 1 || d.nmat > 3 || d.K <= 0 || d.K % 256 || d.K > FLOW_MAX_K) return false;
     if (d.norm_w && (d.K > FLOW_MAX_NORM_K || (reinterpret_cast<uintptr_t>(d.norm_w) & 15))) return false;
@@ -1625,6 +1749,20 @@ bool FlowBuilder::add_matvec(const MatvecDesc & d) {
     }
     if (d.mode == 2) m.R[1] = m.R[0];
     m.x = vec(d.x);
+    // Q8_K hand-over (q8k_block_of): x is a SwiGLU output of this segment and nothing is applied to it before the Q8_K rounding.  The
+    // producer phase, already recorded, is patched to emit the blocks too (a second reader of the same output shares them).
+    const size_t xp = seg_start_ + m.x.tag - 1;                       // the phase that produced x
+    if (d.norm_w == nullptr && m.x.ll != nullptr && xp < phases_.size()) {
+        FlowPhase & pp = phases_[xp];
+        FlowMatvec & pm = pp.mv;
+        if (pp.kind == FLOW_MATVEC && pm.mode == 2 && pm.out[0].ll == m.x.ll && pm.M[0] == d.K && q8k_one_quantiser_per_block(pm, grid_)) {
+            if (!(pm.plan_pad_[0] & FLOW_MV_Q8K_OUT)) {
+                uint64_t * q = carve((size_t)FL_Q8K_WORDS * nblk);
+                if (q != nullptr) { pm.out[1].plain = nullptr; pm.out[1].ll = q; pm.plan_pad_[0] |= FLOW_MV_Q8K_OUT; }
+            }
+            if (pm.plan_pad_[0] & FLOW_MV_Q8K_OUT) { m.x.ll = pm.out[1].ll; m.x.flags |= FLOW_VEC_Q8K; }
+        }
+    }
     if (d.mode == 1) {
         m.resid_h = (h_ptr_ != nullptr && (d.residual == h_ptr_ || d.residual == h_ptr_copy_) && d.M[0] <= FLOW_MAX_H) ? 1 : 0;
         m.residual = vec(d.residual);
