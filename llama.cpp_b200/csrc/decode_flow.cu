@@ -41,7 +41,6 @@
 // All spin loops are bounded and __trap(): a lost producer must fail the launch, never hang the GPU.
 #include <cuda_fp16.h>
 #include <stdio.h>
-#include <stdlib.h>
 #include <string.h>
 
 #include "decode_flow.cuh"
@@ -51,9 +50,6 @@ namespace qmm {
 
 namespace {
 
-#ifndef FLOW_TP
-#define FLOW_TP 0
-#endif
 constexpr int FL_NW = 7;                                   // consumer warps (7 + the producer = 256 threads: the full 255-register budget).  Tried:
                                                            // 9 warps (allocated like 12: 168 registers, spills); 8 consumer warps + a producer
                                                            // warpgroup with setmaxnreg 232 / 40 (550 bytes of spills; did not complete the 8B run
@@ -62,11 +58,7 @@ constexpr int FL_PROD_WARPS = 1;
 constexpr int FL_NPAIR = FL_NW / 2;                       // warp pairs when a row is split over two warps (K > 8192)
 constexpr int FL_CTHREADS = FL_NW * 32;
 constexpr int FL_THREADS = FL_CTHREADS + 32 * FL_PROD_WARPS;   // + the producer warp(group)
-#if defined(FLOW_AB_NSLOTS)
-constexpr int FL_NSLOTS = FLOW_AB_NSLOTS;                  // (14 slots: the CTA fits the 196 KB shared-memory configuration and leaves 32 KB of L1 for the spills)
-#else
 constexpr int FL_NSLOTS = 18;
-#endif
 constexpr int FL_SLOT = 9728;                              // bytes per ring slot (multiple of 128)
 constexpr int FL_MAXBLK = FLOW_MAX_K / 256;                // 64
 constexpr int FL_PU = 5;                                   // activation blocks per warp and prologue pass
@@ -140,21 +132,9 @@ __device__ __forceinline__ void fl_mbar_wait(uint64_t * bar, uint32_t parity) {
         if ((++n & 63) == 0 && gtime() - t0 > 4000000000ull) __trap();
     }
 }
-// Tags are relative to an epoch that lives in device memory and only grows.  Single GPU: one epoch (phases of this launch).  The
-// tensor-parallel build (FLOW_TP, decode_flow_tp.cu) adds the collective epoch of the GPU group for vectors written by peers.
-#if FLOW_TP
-struct EpochT { uint32_t phase, coll; };
-__device__ __forceinline__ uint32_t want_tag(const FlowVec & v, const EpochT & ep) { return ((v.flags & FLOW_VEC_COLL) ? ep.coll : ep.phase) + v.tag; }
-__device__ __forceinline__ uint32_t phase_epoch(const EpochT & ep) { return ep.phase; }
-__device__ __forceinline__ void st_slot_sys(uint64_t * p, uint32_t tag, float v) {       // a peer GPU's memory, over NVLink
-    const uint64_t w = ((uint64_t)tag << 32) | (uint64_t)__float_as_uint(v);
-    asm volatile("st.relaxed.sys.global.u64 [%0], %1;\n" ::"l"(p), "l"(w) : "memory");
-}
-#else
+// Tags are relative to an epoch that lives in device memory and only grows: a slot is valid at epoch + producer phase + 1.
 typedef uint32_t EpochT;
 __device__ __forceinline__ uint32_t want_tag(const FlowVec & v, EpochT ep) { return ep + v.tag; }
-__device__ __forceinline__ uint32_t phase_epoch(EpochT ep) { return ep; }
-#endif
 // one element of a vector (polls while the producer has not written it)
 __device__ __forceinline__ float vec_ld(const FlowVec & v, int i, EpochT epoch) {
     if (v.ll != nullptr) {
@@ -222,19 +202,6 @@ __device__ __forceinline__ void vec_ld8_finish_blocks(const FlowVec & v, const i
     if (v.ll != nullptr) {
         const uint32_t want = want_tag(v, epoch);
         long long spins = 0;
-#if defined(FLOW_AB_SEQ_POLL)
-#pragma unroll
-        for (int u = 0; u < NU; u++) {
-            if (!on[u]) continue;
-#pragma unroll
-            for (int c = 0; c < 4; c++) {
-                while ((uint32_t)(raw[u][2 * c] >> 32) != want || (uint32_t)(raw[u][2 * c + 1] >> 32) != want) {
-                    spin_fail(spins);
-                    ld_slot2(v.ll + idx[u] + 2 * c, raw[u][2 * c], raw[u][2 * c + 1]);
-                }
-            }
-        }
-#else
         if (on[0]) {                                                  // (block 0 of a pass exists for every warp that has any block in it)
             while ((uint32_t)(raw[0][0] >> 32) != want || (uint32_t)(raw[0][1] >> 32) != want) {
                 spin_fail(spins);
@@ -260,7 +227,6 @@ __device__ __forceinline__ void vec_ld8_finish_blocks(const FlowVec & v, const i
             if (!stale) break;
             spin_fail(spins);
         }
-#endif
     }
 #pragma unroll
     for (int u = 0; u < NU; u++) {
@@ -447,113 +413,15 @@ __device__ __forceinline__ int next_matvec(const FlowPhase * __restrict__ ph, in
     while (from < n_phases && __ldg(&ph[from].kind) != FLOW_MATVEC) from++;
     return from;
 }
-#if defined(FLOW_AB_SERIAL_PRODUCER)
-__device__ __forceinline__ void producer_loop(const FlowPhase * __restrict__ ph, int n_phases, uint8_t * smem, int lane, int throttle) {
-    uint64_t * full = reinterpret_cast<uint64_t *>(smem + OFF_BARS), * empty = full + FL_NSLOTS;
-    uint8_t * ring = smem + OFF_RING;
-    uint32_t * pdesc = reinterpret_cast<uint32_t *>(smem + OFF_DESC + 2 * 384);
-    const int cta = (int)blockIdx.x, grid = (int)gridDim.x;
-    unsigned g = 0;                                                  // pieces issued so far (this CTA, whole program)
-    const uint64_t l2_pol = l2_evict_first_policy();                 // evict-first weight stream: see the header
-    int pi = next_matvec(ph, 0, n_phases), buf = 0;
-    if (pi < n_phases) {
-        const uint32_t * src = reinterpret_cast<const uint32_t *>(ph + pi);
-        for (int i = lane; i < DESC_WORDS; i += 32) pdesc[i] = __ldg(src + i);
-    }
-    __syncwarp();
-    while (pi < n_phases) {
-        const int pn = next_matvec(ph, pi + 1, n_phases);
-        uint32_t nxt[(DESC_WORDS + 31) / 32];
-        if (pn < n_phases) {
-            const uint32_t * src = reinterpret_cast<const uint32_t *>(ph + pn);
-#pragma unroll
-            for (int i = 0; i < (DESC_WORDS + 31) / 32; i++) if (lane + 32 * i < DESC_WORDS) nxt[i] = __ldg(src + lane + 32 * i);
-        }
-        const FlowMatvec & p = reinterpret_cast<const FlowPhase *>(pdesc + buf * 96)->mv;
-        const int nblk = p.K >> 8, S = p.S, seg = p.seg;
-        const int nenum = p.mode == 2 ? 1 : p.nmat, sub = p.mode == 2 ? 2 : 1;
-        for (int m = 0; m < nenum; m++) {
-            // per-matrix constants in registers (the piece loop below must be lean: it has to stay ahead of 7 consumer warps)
-            const int Mm = p.M[m], R = p.R[m], bb = block_bytes(p.type[m]);
-            const int rb = row_begin(p, m, cta), re = row_begin(p, m, cta + 1);
-            const int row_bytes = nblk * bb;
-            const uint8_t * w0 = p.w[m], * w1 = p.w[1];
-            const int64_t rs0 = p.row_stride[m], rs1 = p.row_stride[1];
-            const bool contiguous = S == 1 && rs0 == (int64_t)row_bytes && (sub == 1 || rs1 == (int64_t)row_bytes);
-            const int spitch = sub_pitch(R, row_bytes), rpitch = row_pitch(seg, bb);
-            for (int r0 = rb; r0 < re; r0 += R) {
-                const int nr = min(R, re - r0);
-                // the piece is one or a few contiguous runs (dense rows: one per sub-piece; otherwise one per row segment); lane rj
-                // copies run rj.  (Cutting runs into smaller chunks issued side by side was measured and is slower: 268 tok/s at
-                // 1 KB chunks, 296 at 4 KB, 343 unchunked -- the copy engine prefers few large copies.)
-                const int nruns = contiguous ? sub : sub * nr;
-                for (int sgm = 0; sgm < S; sgm++) {
-                    const unsigned slot = g % FL_NSLOTS, use = g / FL_NSLOTS;
-                    if (use > 0) fl_mbar_wait(empty + slot, (use - 1) & 1u);
-                    if (throttle > 0 && g >= (unsigned)throttle) {   // at most `throttle` pieces in flight: keeps the SM's memory queue short
-                        const unsigned og = g - (unsigned)throttle;
-                        fl_mbar_wait(full + og % FL_NSLOTS, (og / FL_NSLOTS) & 1u);
-                    }
-                    uint8_t * sl = ring + (size_t)slot * FL_SLOT;
-                    const uint8_t * src = nullptr;
-                    uint8_t * dst = nullptr;
-                    uint32_t cnt = 0;
-                    if (lane < nruns) {
-                        const uint8_t * gp;
-                        uint32_t total;
-                        if (contiguous) {
-                            gp = (sub == 2 && lane == 1 ? w1 : w0) + (int64_t)r0 * (sub == 2 && lane == 1 ? rs1 : rs0);
-                            dst = sl + lane * spitch;
-                            total = (uint32_t)(nr * row_bytes);
-                        } else {
-                            const int j = lane >= nr ? 1 : 0, r = lane - j * nr;
-                            gp = (sub == 2 && j ? w1 : w0) + (int64_t)(r0 + r) * (sub == 2 && j ? rs1 : rs0) + (int64_t)sgm * seg * bb;
-                            dst = sl + (j * R + r) * rpitch;
-                            total = (uint32_t)(seg_len(p, nblk, sgm) * bb);
-                        }
-                        const uint32_t off = (uint32_t)(reinterpret_cast<uintptr_t>(gp) & 15);
-                        cnt = (off + total + 15u) & ~15u;
-                        src = gp - off;
-                    }
-                    uint32_t tx = cnt;
-                    if (nruns <= 2) {
-                        tx += __shfl_xor_sync(0xffffffffu, tx, 1);
-                    } else {
-#pragma unroll
-                        for (int o = 16; o > 0; o >>= 1) tx += __shfl_xor_sync(0xffffffffu, tx, o);
-                    }
-                    if (lane == 0) mbar_expect_tx(full + slot, tx);
-                    __syncwarp();
-                    if (cnt) bulk_g2s_hint(dst, src, cnt, full + slot, l2_pol);
-                    g++;
-                }
-            }
-        }
-        // hand over to the next mat-vec phase: its descriptor has long arrived
-        if (pn < n_phases) {
-#pragma unroll
-            for (int i = 0; i < (DESC_WORDS + 31) / 32; i++) if (lane + 32 * i < DESC_WORDS) pdesc[(buf ^ 1) * 96 + lane + 32 * i] = nxt[i];
-        }
-        __syncwarp();
-        buf ^= 1;
-        pi = pn;
-    }
-}
-
-#else
 // What the trace and the bulk-copy micro-benchmark showed together (profiles/r02_flow_trace.md, r02_ubench.md): one lane streaming 9 KB
 // copies saturates HBM, yet every mat-vec phase advanced at one ring piece per ~560 - 710 cycles whatever the piece size (Q6_K pieces of
-// 6.7 KB: 2.7 TB/s, Q4_K pieces of 9.2 KB: 3.8 - 4.6 TB/s).  That is the latency of ONE trip through the serial producer loop (barrier
-// wait, address arithmetic, shuffles, expect_tx, copy).  So FL_PL lanes now walk FL_PL consecutive pieces side by side: each lane
-// decodes its own piece (matrix, row chunk, k-segment), waits for its own slot and issues that piece's copies itself.  The numbering of
-// the pieces (matrix-major, then row chunk, then segment) is unchanged, so the consumers need no change.
-#if defined(FLOW_AB_PL)
-constexpr int FL_PL = FLOW_AB_PL;
-#else
+// 6.7 KB: 2.7 TB/s, Q4_K pieces of 9.2 KB: 3.8 - 4.6 TB/s).  That is the latency of ONE trip through a producer loop that issues the
+// pieces one after the other (barrier wait, address arithmetic, shuffles, expect_tx, copy).  So FL_PL lanes walk FL_PL consecutive
+// pieces side by side (B200: 416 tok/s against 378 for the serial loop): each lane decodes its own piece (matrix, row chunk, k-segment),
+// waits for its own slot and issues that piece's copies itself.  Pieces are numbered matrix-major, then row chunk, then segment, the
+// order in which the consumers take them.
 constexpr int FL_PL = 8;
-#endif
-__device__ __forceinline__ void producer_loop(const FlowPhase * __restrict__ ph, int n_phases, uint8_t * smem, int lane, int throttle) {
-    (void)throttle;
+__device__ __forceinline__ void producer_loop(const FlowPhase * __restrict__ ph, int n_phases, uint8_t * smem, int lane) {
     uint64_t * full = reinterpret_cast<uint64_t *>(smem + OFF_BARS), * empty = full + FL_NSLOTS;
     uint8_t * ring = smem + OFF_RING;
     uint32_t * pdesc = reinterpret_cast<uint32_t *>(smem + OFF_DESC + 2 * 384);
@@ -600,7 +468,8 @@ __device__ __forceinline__ void producer_loop(const FlowPhase * __restrict__ ph,
                 if (use > 0) fl_mbar_wait(empty + slot, (use - 1) & 1u);
                 uint8_t * sl = ring + (size_t)slot * FL_SLOT;
                 if (contiguous) {
-                    // dense rows: one copy per sub-piece (SwiGLU: gate rows, up rows)
+                    // dense rows: one copy per sub-piece (SwiGLU: gate rows, up rows).  Cutting it into smaller copies issued side by side
+                    // measured slower (B200: 268 tok/s at 1 KB, 296 at 4 KB, 343 uncut): the copy engine prefers few large copies.
                     const uint8_t * g0 = w0 + (int64_t)r0 * rs0, * g1 = w1 + (int64_t)r0 * rs1;
                     const uint32_t total = (uint32_t)(nr * row_bytes);
                     const uint32_t off0 = (uint32_t)(reinterpret_cast<uintptr_t>(g0) & 15), off1 = (uint32_t)(reinterpret_cast<uintptr_t>(g1) & 15);
@@ -641,7 +510,6 @@ __device__ __forceinline__ void producer_loop(const FlowPhase * __restrict__ ph,
         pi = pn;
     }
 }
-#endif
 
 // ------------------------------------------------------------------------------------------------ Q8_K quantisation of one 256-block held by a warp
 // quantize_row_q8_K_ref (ggml-quants.c:2768-2805): lane l holds elements 8l..8l+7; the FIRST element of largest magnitude decides
@@ -674,7 +542,8 @@ __device__ __forceinline__ void quant_lane(const float (&v)[8], uint2 & packed, 
     const int s8 = q[0] + q[1] + q[2] + q[3] + q[4] + q[5] + q[6] + q[7];
     s16 = s8 + __shfl_xor_sync(0xffffffffu, s8, 1);
 }
-// ... written to the prologue's shared-memory layout: the int8 values (skewed pitch), the 16 sums of 16 and the scale of block b
+// ... written to the prologue's shared-memory layout: the int8 values (skewed pitch), the 16 sums of 16 and the scale of block b.
+// One block at a time: interleaving several blocks' quantisers measured slower (B200: 420 vs 426 tok/s, the extra live registers).
 __device__ __forceinline__ void quant_block(const float (&v)[8], int b, int lane, uint8_t * act) {
     uint2 packed;
     int s16;
@@ -695,59 +564,6 @@ __device__ __forceinline__ void quant_block_ll(const float (&v)[8], int b, int n
     const int s16_next = __shfl_down_sync(0xffffffffu, s16, 2);      // the next group's sum: two groups per word
     if ((lane & 3) == 0) st_word(ll + 64 * nblk + 8 * b + (lane >> 2), tag, ((uint32_t)s16 & 0xFFFFu) | ((uint32_t)s16_next << 16));
     if (lane == 0) st_word(ll + 72 * nblk + b, tag, __float_as_uint(d));
-}
-
-// (FLOW_AB_BATCH_QUANT builds only: measured 420 vs 426 tok/s for the serial form, lease X -- the extra live registers cost more than the
-// overlapped chains gain.)  The same for NU blocks at once, stage by stage: one block is a serial latency chain (redux -> ballot -> shuffle -> IEEE division ->
-// convert -> division -> pack -> store, ~500 cycles) and a warp quantises 3 - 8 blocks per phase while 147 other CTAs wait for nobody
-// but themselves -- the fine-grained trace put 2.0 us (K = 4096) and 5.3 us (K = 14336) of every dependency hop here.  With the
-// stages of the NU blocks interleaved the chains overlap.  Same arithmetic, bit for bit (blocks that do not exist compute on zeros and
-// store nothing).
-template <int NU>
-__device__ __forceinline__ void quant_blocks(const float (&v)[NU][8], const int (&b)[NU], const bool (&on)[NU], int lane, uint8_t * act) {
-    unsigned mloc[NU], mall[NU];
-#pragma unroll
-    for (int u = 0; u < NU; u++) {
-        mloc[u] = 0;
-#pragma unroll
-        for (int i = 0; i < 8; i++) { const unsigned a = (v[u][i] == v[u][i]) ? (__float_as_uint(v[u][i]) & 0x7fffffffu) : 0u; mloc[u] = a > mloc[u] ? a : mloc[u]; }
-    }
-#pragma unroll
-    for (int u = 0; u < NU; u++) mall[u] = __reduce_max_sync(0xffffffffu, mloc[u]);
-    float mine[NU], maxv[NU];
-    int wl[NU];
-#pragma unroll
-    for (int u = 0; u < NU; u++) {
-        wl[u] = __ffs((int)__ballot_sync(0xffffffffu, mloc[u] == mall[u])) - 1;
-        mine[u] = 0.0f;
-#pragma unroll
-        for (int i = 7; i >= 0; i--) mine[u] = ((__float_as_uint(v[u][i]) & 0x7fffffffu) == mall[u] && v[u][i] == v[u][i]) ? v[u][i] : mine[u];
-    }
-#pragma unroll
-    for (int u = 0; u < NU; u++) maxv[u] = __shfl_sync(0xffffffffu, mine[u], wl[u]);
-    float iscale[NU], d[NU];
-#pragma unroll
-    for (int u = 0; u < NU; u++) {
-        const bool nz = __uint_as_float(mall[u]) > 0.0f;
-        iscale[u] = nz ? __fdiv_rn(-127.0f, maxv[u]) : 0.0f;            // (all-zero block: every q becomes 0, d = 0)
-        d[u] = nz ? __fdiv_rn(1.0f, iscale[u]) : 0.0f;
-    }
-#pragma unroll
-    for (int u = 0; u < NU; u++) {
-        int q[8];
-#pragma unroll
-        for (int i = 0; i < 8; i++) { const int t = __float2int_rn(__fmul_rn(iscale[u], v[u][i])); q[i] = t > 127 ? 127 : t; }
-        uint2 packed;
-        packed.x = (uint32_t)(q[0] & 0xFF) | ((uint32_t)(q[1] & 0xFF) << 8) | ((uint32_t)(q[2] & 0xFF) << 16) | ((uint32_t)(q[3] & 0xFF) << 24);
-        packed.y = (uint32_t)(q[4] & 0xFF) | ((uint32_t)(q[5] & 0xFF) << 8) | ((uint32_t)(q[6] & 0xFF) << 16) | ((uint32_t)(q[7] & 0xFF) << 24);
-        const int s8 = q[0] + q[1] + q[2] + q[3] + q[4] + q[5] + q[6] + q[7];
-        const int s16 = s8 + __shfl_xor_sync(0xffffffffu, s8, 1);
-        if (on[u]) {
-            *reinterpret_cast<uint2 *>(act + (size_t)b[u] * ACT_PITCH + 8 * lane) = packed;
-            if ((lane & 1) == 0) reinterpret_cast<int16_t *>(act + ACT_BS + (size_t)b[u] * 32)[lane >> 1] = (int16_t)s16;
-            if (lane == 0) reinterpret_cast<float *>(act + ACT_D)[b[u]] = d[u];
-        }
-    }
 }
 
 // The prologue of a mat-vec whose input is a Q8_K vector: every consumer thread issues all of its 16-byte loads of the blocks' words at
@@ -826,9 +642,6 @@ struct MatCtx {
     bool contiguous;
     uint32_t tag;
     EpochT epoch;
-#if FLOW_TP
-    const FlowMatvec * desc;           // shared-memory descriptor (peer pointers of a tensor-parallel partial result)
-#endif
 };
 
 __device__ __forceinline__ void mv_epilogue(const MatCtx & mc, int row, float v, float gate) {
@@ -838,13 +651,6 @@ __device__ __forceinline__ void mv_epilogue(const MatCtx & mc, int row, float v,
     } else {
         if (mc.mode == 1) v = __fadd_rn(v, mc.h != nullptr ? mc.h[row] : vec_ld(mc.residual, row, mc.epoch));
         out_st(mc.out, row, mc.tag, v);
-#if FLOW_TP
-        const int npeer = mc.desc->npeer;
-        if (npeer > 0) {                                       // tensor-parallel partial: one tagged slot per GPU of the group, over NVLink
-            const uint32_t ctag = mc.epoch.coll + mc.desc->coll + 1u;
-            for (int d = 0; d < npeer; d++) st_slot_sys(mc.desc->peer[d] + row, ctag, v);
-        }
-#endif
     }
 }
 
@@ -932,7 +738,7 @@ __device__ __forceinline__ void matvec_phase(const FlowMatvec & p, int pi, Ctx &
     const int cta = (int)blockIdx.x, grid = (int)gridDim.x;
     const int nblk = p.K >> 8;
     const EpochT epoch = c.epoch;
-    const uint32_t tag = phase_epoch(epoch) + (uint32_t)pi + 1u;
+    const uint32_t tag = epoch + (uint32_t)pi + 1u;
     uint8_t * act = smem + OFF_ACT;
     double * red = reinterpret_cast<double *>(smem + OFF_RED);
     float * part = reinterpret_cast<float *>(smem + OFF_PART);
@@ -977,21 +783,6 @@ __device__ __forceinline__ void matvec_phase(const FlowMatvec & p, int pi, Ctx &
             vec_ld8_finish_blocks<FL_PU>(p.x, idx, on, epoch, raw, xv);
 #endif
         }
-        // the norm weights of this warp's blocks: requested now, so that their L2 round trip runs under the sum-of-squares reduction
-        // and its barrier (there is practically no L1 next to 227 KB of shared memory)
-#if defined(FLOW_AB_NW_EARLY)
-        float4 nw[FL_PU][2];
-        if (norm) {
-#pragma unroll
-            for (int u = 0; u < FL_PU; u++) {
-                const int b = base + warp + u * FL_NW;
-                if (b < nblk) {
-                    nw[u][0] = __ldg(reinterpret_cast<const float4 *>(p.norm_w + 256 * b + 8 * lane));
-                    nw[u][1] = __ldg(reinterpret_cast<const float4 *>(p.norm_w + 256 * b + 8 * lane) + 1);
-                }
-            }
-        }
-#endif
 #pragma unroll
         for (int u = 0; u < FL_PU; u++) {
             const int b = base + warp + u * FL_NW;
@@ -1023,7 +814,6 @@ __device__ __forceinline__ void matvec_phase(const FlowMatvec & p, int pi, Ctx &
             if (base == 0) stamp(c, pi, 7);
 #endif
         }
-#if !defined(FLOW_AB_BATCH_QUANT)
         {
 #pragma unroll
             for (int u = 0; u < FL_PU; u++) {
@@ -1031,11 +821,7 @@ __device__ __forceinline__ void matvec_phase(const FlowMatvec & p, int pi, Ctx &
                 if (b < nblk) {
                     float v[8];
                     if (norm) {
-#if defined(FLOW_AB_NW_EARLY)
-                        const float4 w0 = nw[u][0], w1 = nw[u][1];
-#else
                         const float4 w0 = __ldg(reinterpret_cast<const float4 *>(p.norm_w + 256 * b + 8 * lane)), w1 = __ldg(reinterpret_cast<const float4 *>(p.norm_w + 256 * b + 8 * lane) + 1);
-#endif
                         const float wv[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
 #pragma unroll
                         for (int i = 0; i < 8; i++) v[i] = __fmul_rn(__fmul_rn(xv[u][i], scale), wv[i]);
@@ -1052,43 +838,6 @@ __device__ __forceinline__ void matvec_phase(const FlowMatvec & p, int pi, Ctx &
                 }
             }
         }
-#else
-        {
-            float v[FL_PU][8];
-            int bi[FL_PU];
-            bool onb[FL_PU];
-#pragma unroll
-            for (int u = 0; u < FL_PU; u++) { bi[u] = base + warp + u * FL_NW; onb[u] = bi[u] < nblk; }
-            if (norm) {
-                float4 w0[FL_PU], w1[FL_PU];
-#pragma unroll
-                for (int u = 0; u < FL_PU; u++) {                        // all the norm-weight loads of the warp go out together
-                    if (onb[u]) {
-                        w0[u] = __ldg(reinterpret_cast<const float4 *>(p.norm_w + 256 * bi[u] + 8 * lane));
-                        w1[u] = __ldg(reinterpret_cast<const float4 *>(p.norm_w + 256 * bi[u] + 8 * lane) + 1);
-                    } else { w0[u] = make_float4(0.f, 0.f, 0.f, 0.f); w1[u] = w0[u]; }
-                }
-#pragma unroll
-                for (int u = 0; u < FL_PU; u++) {
-                    const float wv[8] = {w0[u].x, w0[u].y, w0[u].z, w0[u].w, w1[u].x, w1[u].y, w1[u].z, w1[u].w};
-#pragma unroll
-                    for (int i = 0; i < 8; i++) v[u][i] = onb[u] ? __fmul_rn(__fmul_rn(xv[u][i], scale), wv[i]) : 0.0f;
-                    if (onb[u] && p.norm_out != nullptr && cta == 0) {
-                        float4 * op = reinterpret_cast<float4 *>(p.norm_out + 256 * bi[u] + 8 * lane);
-                        op[0] = make_float4(v[u][0], v[u][1], v[u][2], v[u][3]);
-                        op[1] = make_float4(v[u][4], v[u][5], v[u][6], v[u][7]);
-                    }
-                }
-            } else {
-#pragma unroll
-                for (int u = 0; u < FL_PU; u++) {
-#pragma unroll
-                    for (int i = 0; i < 8; i++) v[u][i] = onb[u] ? xv[u][i] : 0.0f;
-                }
-            }
-            quant_blocks<FL_PU>(v, bi, onb, lane, act);
-        }
-#endif
     }
 #if defined(FLOW_FINE_TRACE)
     stamp(c, pi, 8);
@@ -1126,9 +875,6 @@ __device__ __forceinline__ void matvec_phase(const FlowMatvec & p, int pi, Ctx &
     MatCtx mc;
     mc.mode = p.mode; mc.S = p.S; mc.seg = p.seg; mc.RP = p.RP; mc.rp_shift = 31 - __clz(p.RP);
     mc.h = hres; mc.part = part; mc.tag = tag; mc.epoch = epoch;
-#if FLOW_TP
-    mc.desc = &p;
-#endif
     mc.residual = p.residual;
     for (int m = 0; m < nenum; m++) {
         const int Mm = p.M[m], T = p.type[m];
@@ -1221,7 +967,7 @@ __device__ __forceinline__ void attn_phase(const FlowAttn & a, int pi, const Ctx
     const int D = a.head_dim;                                         // 128 (checked on the host)
     if (cta >= a.n_head * nsplit) return;
     const EpochT epoch = c.epoch;
-    const uint32_t tag = phase_epoch(epoch) + (uint32_t)pi + 1u;
+    const uint32_t tag = epoch + (uint32_t)pi + 1u;
     const int h = cta / nsplit, part = cta % nsplit;
     const int gqa = a.n_head / a.n_head_kv, hk = h / gqa;
     float * att = reinterpret_cast<float *>(smem + OFF_ACT);
@@ -1252,15 +998,6 @@ __device__ __forceinline__ void attn_phase(const FlowAttn & a, int pi, const Ctx
     const int dc = tid & 15, kg = tid >> 4;                           // P.V ownership: dims 8dc..8dc+7, keys kg, kg + FL_KG, ...
     const int key_pf = k0 + tid;
     const float mv_pf = (mp && key_pf < k1) ? __half2float(mp[key_pf]) : 0.0f;
-#if defined(FLOW_AB_ATTN_PREFETCH_V)
-    uint4 vpf[8];
-#pragma unroll
-    for (int u = 0; u < 8; u++) {
-        const int key = k0 + kg + u * FL_KG;
-        vpf[u] = make_uint4(0u, 0u, 0u, 0u);
-        if (key < k1 && key != (int)vpos) vpf[u] = __ldg(reinterpret_cast<const uint4 *>(vbase + (int64_t)key * a.v_nb1) + dc);
-    }
-#endif
     // every load of this thread goes out first (q pair, k pair, v element), then whatever is still stale is re-polled as a batch: the three
     // vectors come from the same mat-vec phase, so they land together and sequential re-polls would only add L2 round trips
     const bool has_v = tid < D;
@@ -1371,6 +1108,7 @@ __device__ __forceinline__ void attn_phase(const FlowAttn & a, int pi, const Ctx
         M = Mnew;
 #pragma unroll
         for (int i = 0; i < 8; i++) o[i] *= alpha;
+        // (requesting the first round's V chunks before the q/k/v wait instead was measured slower: DESIGN 5.3)
         for (int key0 = t0 + kg; key0 < t1; key0 += 8 * FL_KG) {     // 8 keys of this thread's group per round: their V chunks in flight together
             float pvv[8];
             uint4 rawv[8];
@@ -1379,9 +1117,6 @@ __device__ __forceinline__ void attn_phase(const FlowAttn & a, int pi, const Ctx
                 const int key = key0 + u * FL_KG;
                 pvv[u] = key < t1 ? sS[key - t0] : 0.0f;
                 rawv[u] = make_uint4(0u, 0u, 0u, 0u);
-#if defined(FLOW_AB_ATTN_PREFETCH_V)
-                if (key0 == k0 + kg) { rawv[u] = vpf[u]; continue; }
-#endif
                 if (pvv[u] != 0.0f && key != (int)vpos) rawv[u] = __ldg(reinterpret_cast<const uint4 *>(vbase + (int64_t)key * a.v_nb1) + dc);
             }
 #pragma unroll
@@ -1444,7 +1179,7 @@ __device__ __forceinline__ void attn_phase(const FlowAttn & a, int pi, const Ctx
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
-__global__ void __launch_bounds__(FL_THREADS, 1) decode_flow_kernel(const FlowPhase * __restrict__ ph, int n_phases, unsigned * sync, unsigned long long * trace, int throttle, int n_coll) {
+__global__ void __launch_bounds__(FL_THREADS, 1) decode_flow_kernel(const FlowPhase * __restrict__ ph, int n_phases, unsigned * sync, unsigned long long * trace) {
     extern __shared__ __align__(128) uint8_t smem[];
     const int tid = (int)threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint64_t * full = reinterpret_cast<uint64_t *>(smem + OFF_BARS), * empty = full + FL_NSLOTS;
@@ -1455,16 +1190,10 @@ __global__ void __launch_bounds__(FL_THREADS, 1) decode_flow_kernel(const FlowPh
     asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
     if (tid < DESC_WORDS) reinterpret_cast<uint32_t *>(smem + OFF_DESC)[tid] = __ldg(reinterpret_cast<const uint32_t *>(ph) + tid);
     __syncthreads();
-#if FLOW_TP
-    EpochT epoch;
-    epoch.phase = __ldcg(sync);                                       // left by the previous launch (0 after allocation)
-    epoch.coll = __ldcg(sync + 2);
-#else
     const EpochT epoch = __ldcg(sync);                                // left by the previous launch (0 after allocation)
-#endif
 
     if (warp >= FL_NW) {
-        if (warp == FL_NW) producer_loop(ph, n_phases, smem, lane, throttle);
+        if (warp == FL_NW) producer_loop(ph, n_phases, smem, lane);
     } else {
         // The consumers read the current phase's descriptor from shared memory (two slots); the next one is fetched at phase entry
         // and parked in a register until the phase's work is done (see producer_loop for why).
@@ -1483,55 +1212,8 @@ __global__ void __launch_bounds__(FL_THREADS, 1) decode_flow_kernel(const FlowPh
                 matvec_phase(d.mv, pi, c, smem);
             } else if (kind == FLOW_ATTN) {
                 attn_phase(d.at, pi, c, smem);
-#if FLOW_TP
-            } else if (kind == FLOW_SUM) {
-                // out = src[0] + src[1] + ... (rank order: bit-identical on every GPU of the group), 8 elements per thread, the vector
-                // spread over all CTAs: the reduce half of the fused all-reduce (and the ADD that follows it, when the host folded it in)
-                const FlowSum & sm = d.sm;
-                const uint32_t tag = phase_epoch(epoch) + (uint32_t)pi + 1u;
-                const int nunits = sm.n >> 3;
-                const int u0 = (int)(((long long)nunits * blockIdx.x) / gridDim.x), u1 = (int)(((long long)nunits * (blockIdx.x + 1)) / gridDim.x);
-                for (int u = u0 + tid; u < u1; u += FL_CTHREADS) {
-                    float acc[8];
-#pragma unroll
-                    for (int k = 0; k < 8; k++) acc[k] = 0.0f;
-                    for (int s0 = 0; s0 < sm.nsrc; s0 += 3) {             // three sources' loads in flight together
-                        uint64_t raw[3][8];
-                        float x[8];
-#pragma unroll
-                        for (int j = 0; j < 3; j++) if (s0 + j < sm.nsrc) vec_ld8_issue(sm.src[s0 + j], 8 * u, raw[j]);
-#pragma unroll
-                        for (int j = 0; j < 3; j++) {
-                            if (s0 + j < sm.nsrc) {
-                                vec_ld8_finish(sm.src[s0 + j], 8 * u, epoch, raw[j], x);
-#pragma unroll
-                                for (int k = 0; k < 8; k++) acc[k] = (s0 + j) == 0 ? x[k] : __fadd_rn(acc[k], x[k]);
-                                if (s0 + j + 1 == sm.n_first) {
-#pragma unroll
-                                    for (int k = 0; k < 8; k++) out_st(sm.out, 8 * u + k, tag, acc[k]);
-                                }
-                            }
-                        }
-                    }
-                    if (sm.n_first < sm.nsrc) {
-#pragma unroll
-                        for (int k = 0; k < 8; k++) out_st(sm.out2, 8 * u + k, tag, acc[k]);
-                    }
-                }
-                if (blockIdx.x == 0) {                                      // ragged tail
-                    for (int i = 8 * nunits + tid; i < sm.n; i += FL_CTHREADS) {
-                        float a = vec_ld(sm.src[0], i, epoch);
-                        if (sm.n_first == 1) out_st(sm.out, i, tag, a);
-                        for (int s1 = 1; s1 < sm.nsrc; s1++) {
-                            a = __fadd_rn(a, vec_ld(sm.src[s1], i, epoch));
-                            if (s1 + 1 == sm.n_first) out_st(sm.out, i, tag, a);
-                        }
-                        if (sm.n_first < sm.nsrc) out_st(sm.out2, i, tag, a);
-                    }
-                }
-#endif
             } else if (blockIdx.x == 0) {
-                const uint32_t tag = phase_epoch(epoch) + (uint32_t)pi + 1u;
+                const uint32_t tag = epoch + (uint32_t)pi + 1u;
                 if (kind == FLOW_COPY) {
                     const FlowCopy & cp = d.cp;
                     for (int i = 8 * tid; i < cp.n; i += 8 * FL_CTHREADS) vec_copy8(cp.src, cp.src, false, cp.out, i, cp.n, tag, epoch);
@@ -1549,10 +1231,7 @@ __global__ void __launch_bounds__(FL_THREADS, 1) decode_flow_kernel(const FlowPh
         __threadfence();
         const unsigned old = atomicAdd(sync + 1, 1u);
         if (old == gridDim.x - 1) {
-            sync[1] = 0u; sync[0] = phase_epoch(epoch) + (unsigned)n_phases + 1u;
-#if FLOW_TP
-            sync[2] = epoch.coll + (unsigned)n_coll;
-#endif
+            sync[1] = 0u; sync[0] = epoch + (unsigned)n_phases + 1u;
             __threadfence();
         }
     }
@@ -1571,19 +1250,11 @@ int sm_count_of(int dev) {
 
 }  // namespace
 
-#ifndef FLOW_SECONDARY
 size_t flow_sync_bytes() { return 256; }
 size_t flow_slot_bytes() { return FL_SLOT; }
 int    flow_grid(int device) { return sm_count_of(device); }
-cudaError_t launch_decode_flow_tp(const FlowProgram & prog, cudaStream_t st);   // decode_flow_tp.cu: the same kernel built with FLOW_TP (peer stores, collective epoch, sum phase)
-#endif
 
-#ifdef FLOW_SECONDARY
-cudaError_t launch_decode_flow_tp(const FlowProgram & prog, cudaStream_t st) {
-#else
 cudaError_t launch_decode_flow(const FlowProgram & prog, cudaStream_t st) {
-    if (prog.n_coll > 0) return launch_decode_flow_tp(prog, st);      // programs with a fused all-reduce need the tensor-parallel build
-#endif
     if (prog.n_phases <= 0) return cudaSuccess;
     int dev = 0;
     cudaGetDevice(&dev);
@@ -1599,11 +1270,8 @@ cudaError_t launch_decode_flow(const FlowProgram & prog, cudaStream_t st) {
         if (e != cudaSuccess) return e;
         if (per_sm < 1) return cudaErrorCooperativeLaunchTooLarge;
         cudaDeviceGetAttribute(&coop[dev & 63], cudaDevAttrCooperativeLaunch, dev);
-        const char * ce = getenv("GGML_B200_FLOW_COOP");
-        if (ce != nullptr && ce[0] == '0') coop[dev & 63] = 0;
         attr[dev & 63] = true;
     }
-    static const int throttle = [] { const char * e = getenv("GGML_B200_FLOW_THROTTLE"); return e ? atoi(e) : 0; }();
     cudaLaunchConfig_t cfg{};
     cfg.gridDim = dim3((unsigned)sm_count_of(dev));
     cfg.blockDim = dim3(FL_THREADS);
@@ -1615,21 +1283,19 @@ cudaError_t launch_decode_flow(const FlowProgram & prog, cudaStream_t st) {
     cfg.attrs = at;
     cfg.numAttrs = 1;
     note_launch();
-    return cudaLaunchKernelEx(&cfg, decode_flow_kernel, prog.phases, prog.n_phases, prog.sync, prog.trace, throttle, prog.n_coll);
+    return cudaLaunchKernelEx(&cfg, decode_flow_kernel, prog.phases, prog.n_phases, prog.sync, prog.trace);
 }
 
-#ifndef FLOW_SECONDARY
 // ================================================================================================ host: program builder
 void FlowBuilder::reset(uint64_t * ll_pool, size_t ll_elems, int grid) {
     phases_.clear();
     produced_.clear();
     h_ptr_ = nullptr; h_ptr_copy_ = nullptr;
-    pool_ = ll_pool; pool_elems_ = ll_elems; head_ = 0; seg_start_ = 0; n_coll_ = 0;
+    pool_ = ll_pool; pool_elems_ = ll_elems; head_ = 0; seg_start_ = 0;
     grid_ = grid > 0 ? grid : 132;
 }
 
 void FlowBuilder::cut() {
-    n_coll_ = 0;
     produced_.clear();
     h_ptr_ = nullptr; h_ptr_copy_ = nullptr;
     seg_start_ = phases_.size();
@@ -1829,52 +1495,12 @@ bool FlowBuilder::add_copy(const float * src, float * dst, int n) {
     return true;
 }
 
-bool FlowBuilder::fuse_allreduce(FlowBuilder * const * fb, int n, float * const * tensors, int nelem, uint64_t * const * xpool, size_t xpool_elems, size_t & xoff) {
-    if (n < 2 || n > FLOW_MAX_PEERS || nelem <= 0 || nelem > 65536) return false;
-    const size_t need = ((size_t)n * nelem + 1) & ~size_t(1);
-    if (xoff + need > xpool_elems) return false;
-    const int coll = fb[0]->n_coll_;
-    for (int d = 0; d < n; d++) {
-        FlowBuilder & b = *fb[d];
-        if (b.phases_.size() <= b.seg_start_ || b.n_coll_ != coll || xpool[d] == nullptr) return false;
-        const FlowPhase & last = b.phases_.back();
-        if (last.kind != FLOW_MATVEC || last.mv.nmat != 1 || last.mv.mode == 2 || last.mv.npeer != 0 || last.mv.M[0] != nelem || last.mv.out[0].plain != tensors[d]) return false;
-    }
-    for (int d = 0; d < n; d++) {
-        FlowBuilder & b = *fb[d];
-        FlowMatvec & mv = b.phases_.back().mv;
-        for (int j = 0; j < n; j++) mv.peer[j] = xpool[j] + xoff + (size_t)d * nelem;     // GPU d's partial lands in slot d of every GPU
-        mv.npeer = n; mv.coll = (uint32_t)coll;
-        FlowPhase ph;
-        memset(&ph, 0, sizeof(ph));
-        ph.kind = FLOW_SUM;
-        for (int s = 0; s < n; s++) {
-            FlowVec & v = ph.sm.src[s];
-            v.plain = nullptr; v.ll = xpool[d] + xoff + (size_t)s * nelem; v.tag = (uint32_t)coll + 1u; v.flags = FLOW_VEC_COLL;
-        }
-        ph.sm.nsrc = n; ph.sm.n = nelem; ph.sm.n_first = n;
-        ph.sm.out = b.out(tensors[d], nelem);              // the reduced vector replaces the partial one under the same name
-        b.phases_.push_back(ph);
-        b.n_coll_++;
-    }
-    xoff += need;
-    return true;
-}
+// The kernel has no tensor-parallel sum phase: every all-reduce is declined and the plugin, whose prebuilt objects still call this, flushes
+// the recorded phases and runs its host-driven all-reduce between per-GPU launches.
+bool FlowBuilder::fuse_allreduce(FlowBuilder * const *, int, float * const *, int, uint64_t * const *, size_t, size_t &) { return false; }
 
 bool FlowBuilder::add_add(const float * a, const float * b, float * dst, int n) {
     if (needs_cut(a) || needs_cut(b) || n <= 0) return false;
-    if (phases_.size() > seg_start_) {
-        // the residual ADD right after a fused all-reduce joins its sum phase as one more source (same order of additions: the reduced
-        // vector first, then the residual) -- one dependency hop less per all-reduce; the reduced vector itself is still written
-        FlowPhase & last = phases_.back();
-        if (last.kind == FLOW_SUM && last.sm.n == n && last.sm.n_first == last.sm.nsrc && last.sm.nsrc < FLOW_MAX_PEERS + 1 &&
-            (last.sm.out.plain == a || last.sm.out.plain == b)) {
-            const float * other = last.sm.out.plain == a ? b : a;
-            last.sm.src[last.sm.nsrc++] = vec(other);
-            last.sm.out2 = out(dst, n);
-            return true;
-        }
-    }
     FlowPhase ph;
     memset(&ph, 0, sizeof(ph));
     ph.kind = FLOW_ADD;
@@ -1883,7 +1509,5 @@ bool FlowBuilder::add_add(const float * a, const float * b, float * dst, int n) 
     phases_.push_back(ph);
     return true;
 }
-
-#endif  // FLOW_SECONDARY
 
 }  // namespace qmm

@@ -302,26 +302,22 @@ def _n_gpus():
     return sum(1 for ln in out.splitlines() if ln.startswith("GPU "))
 
 
-@pytest.mark.parametrize("cfg", [pytest.param("fused", marks=pytest.mark.skip(reason=(
-    "known issue (DESIGN.md sections 7, 9): the all-reduce fused into the decode kernel (opt-in, GGML_B200_TP_FUSION=1) traps a launch on two GPUs "
-    "when the whole token is one program per GPU; not run until that trap is diagnosed and fixed"))), "host_allreduce"])
+@pytest.mark.parametrize("cfg", ["host_allreduce"])
 def test_tensor_parallel_two_gpus_match_one(tmp_path, cfg):
     """-sm tensor over two GPUs (the reference's meta backend drives one backend instance per GPU and calls our
     comm_allreduce_tensor hook after every row-split mat-mul) against the same model on one GPU.  The partial sums are added in a
     different order than a single GPU's row reduction; on this random-init model that costs NMSE 3e-4 .. 4e-4 per step (measured, both
     engines; the reference's own two CPU attention paths differ by 7e-4 on it), so the bar is 1e-3 (the reference's test-llama-archs.cpp:671
-    uses 1e-4 on its own tiny models), plus bit-identical logits between two runs of the same configuration.  "fused" (opt-in): the
-    all-reduce is part of the persistent decode kernel (peer stores over NVLink + a sum phase); "host_allreduce" (default): the stand-alone
-    one-shot all-reduce kernel between per-GPU launches of the persistent kernel."""
+    uses 1e-4 on its own tiny models), plus bit-identical logits between two runs of the same configuration.  "host_allreduce": the
+    stand-alone one-shot all-reduce kernel between per-GPU launches of the persistent kernel."""
     if _n_gpus() < 2:
         pytest.skip("needs two GPUs")
     gguf = str(tmp_path / "small.gguf")
     _make_gguf(gguf, "small", "q4_k_m")
     toks = np.random.default_rng(11).integers(0, 512, size=16)
-    extra = {} if cfg == "host_allreduce" else {"GGML_B200_TP_FUSION": "1"}          # host-driven all-reduce is the default
     one = _run_model(gguf, 99, 1, toks, n_decode=8)
-    two = _run_model(gguf, 99, 1, toks, extra, n_decode=8, split_mode=3)
-    again = _run_model(gguf, 99, 1, toks, extra, n_decode=8, split_mode=3)
+    two = _run_model(gguf, 99, 1, toks, n_decode=8, split_mode=3)
+    again = _run_model(gguf, 99, 1, toks, n_decode=8, split_mode=3)
     assert np.isfinite(two).all()
     assert np.array_equal(two, again), np.abs(two - again).max(axis=1)
     per_step = [float(((two[i] - one[i]) ** 2).sum() / (one[i] ** 2).sum()) for i in range(len(one))]

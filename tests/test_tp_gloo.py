@@ -3,8 +3,8 @@
 
   column-parallel (attn_q|k|v, ffn_gate|up): every rank owns M / n weight ROWS; outputs are concatenated -- exact.
   row-parallel (attn_output, ffn_down): every rank owns K / n of every row (a multiple of the 256-weight block, so the Q8_K activation blocks
-      and their integers are those of the full product), computes a partial [N, M] and the partials are ALL-REDUCED.  Our engines add the
-      partials in rank order on every rank (allreduce.cu, decode_flow.cu FLOW_SUM), so every rank holds the same bits; against the
+      and their integers are those of the full product), computes a partial [N, M] and the partials are ALL-REDUCED.  The one-shot
+      all-reduce (allreduce.cu) adds the partials in rank order on every rank, so every rank holds the same bits; against the
       single-device product only the fp32 summation order differs.
 
 The ranks run the oracle on their slice, gloo carries the all-reduce / all-gather -- the same plumbing bench.py --gpus N uses between its ranks."""
@@ -48,7 +48,7 @@ def _worker(rank, world, port, t, M, K, N, out_path):
     dist.all_gather(gathered, partial)
     acc = gathered[0].clone()
     for r in range(1, world):
-        acc = acc + gathered[r]                            # rank order, like the one-shot engine and the FLOW_SUM phase
+        acc = acc + gathered[r]                            # rank order, like the one-shot all-reduce
     row = acc.numpy()
     # every rank must hold the same bits
     chk = torch.from_numpy(row.copy())
